@@ -143,7 +143,7 @@ def load_library(path=None):
     if not os.path.exists(path):
         raise AieError(
             "CUDA extension %s not found. Build it first: `python -c \"import __graft_entry__ as g; g.build()\"` "
-            "(nvcc, sm_100a). There is no CPU fallback." % path)
+            "(nvcc, sm_90a). There is no CPU fallback." % path)
     L = C.CDLL(path)
     P = C.c_void_p
     L.aie_last_error.restype = C.c_char_p

@@ -1,4 +1,4 @@
-"""Compile the CUDA library in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Compile the CUDA library in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import subprocess
 
@@ -7,7 +7,7 @@ LIB = os.path.join(CSRC, "libaie_b200.so")
 SOURCES = ["aie_abi.cu", "aie_expand_host.cpp"]
 DEPS = ["aie_abi.cu", "aie_expand_host.cpp", "aie_abi.inl", "aie_core.cuh", "aie_obs.cuh", "aie_host.h", "aie_layout.h", "aie_covid_core.cuh", "aie_covid_abi.inl", "aie_compact.cuh", "aie_compact_host.h",
         "../../include/aie_b200.h"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
               "-shared", "-Xcompiler", "-fPIC"]
 
 

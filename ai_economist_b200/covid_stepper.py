@@ -72,8 +72,7 @@ class CovidStepperBase:
 
     def __init__(self, params, n_envs, lib, device_index=0, auto_reset=True, change_list=None):
         # change_list: keep a persistent per-state list of stringency changes (O(changes) unemployment response instead
-        # of a history scan).  Default ON: timed on a B200 in round 2 (4 096 envs: 0.065 ms/step against 0.125 ms for the scan,
-        # profiles/r02a_variants.log); AIE_COVID_CHANGE_LIST=0 selects the scan.
+        # of a history scan, whose cost grows with the episode).  Default ON; AIE_COVID_CHANGE_LIST=0 selects the scan.
         if change_list is None:
             import os
             change_list = os.environ.get("AIE_COVID_CHANGE_LIST", "1") not in ("", "0")

@@ -1,4 +1,4 @@
-// aie_abi.cu — CUDA backend of the C-ABI (the product).  sm_100a only; there is no CPU path.
+// aie_abi.cu — CUDA backend of the C-ABI (the product).  sm_90a only; there is no CPU path.
 //
 // Kernels (see DESIGN.md for the roofline of each):
 //   aie_step_kernel        one warp per env replica.  The env's packed state record is staged HBM -> shared
@@ -388,9 +388,11 @@ int check_device(int device) {
         return fail(AIE_ECUDA, std::string("no CUDA device: this library has no CPU fallback (") +
                                    (e == cudaSuccess ? "device count 0" : cudaGetErrorString(e)) + ")");
     if (device < 0 || device >= ndev) return fail(AIE_EINVAL, "device ordinal out of range");
-    int major = 0;
+    int major = 0, minor = 0;
     AIE_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device), "cudaDeviceGetAttribute");
-    if (major < 10) return fail(AIE_ECUDA, "this build targets sm_100a (Blackwell B200) only");
+    AIE_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device), "cudaDeviceGetAttribute");
+    // sm_90a code runs on compute capability 9.0 and nothing else (arch-specific targets are not forward compatible)
+    if (major != 9 || minor != 0) return fail(AIE_ECUDA, "this build targets sm_90a (Hopper H100) only");
     return AIE_OK;
 }
 
@@ -422,9 +424,10 @@ int init(aie_env *env) {
     env->be.step_smem = cta_smem(wpb);
     env->be.obs_threads = wpb * 32;
     env->be.obs_smem = env->be.step_smem;
-    // Register budget: the 64-register variant (launch bounds 256 x 4) when more than 24 warps can be resident - measured
-    // fastest on B200 for c2 (32 warps: 151 us; 24 warps at 80 registers 182 us; 40 warps at 48 registers 213 us) -
-    // otherwise the 80-register variant, which does not spill.  Override: AIE_STEP_MINB=3|4|5.
+    // Register budget: the 64-register variant (launch bounds 256 x 4) when more than 24 warps can be resident (c2: 32
+    // warps per SM), otherwise the 80-register variant, which does not spill.  Override: AIE_STEP_MINB=3|4|5.  This rule
+    // and the envs-per-CTA search above are carried over from the kernels' first target (same 228 KB of shared memory and
+    // 64 K registers per SM as the H100); they have not been re-tuned on the H100.
     const size_t smem_sm = prop.sharedMemPerMultiprocessor;
     int fit = (int)(smem_sm / (env->be.step_smem + 1024));
     const int resident_warps = (fit * wpb > 32) ? 32 : fit * wpb;
@@ -497,8 +500,8 @@ int compact_buffers(aie_env *env, size_t bytes, uint8_t **dev, uint8_t **host) {
         env->be.compact_dev = nullptr; env->be.compact_bytes = 0;
         AIE_CUDA(cudaMalloc((void **)&env->be.compact_dev, bytes), "cudaMalloc compact buffer");
         // AIE_E2E_STAGING_NODE: -1 (default) plain cudaHostAlloc, k >= 0 pages bound to NUMA node k, -2 the node the GPU
-        // hangs off.  No placement was reliably faster than the plain allocation on the B200 host (the staging traffic is
-        // 7 % of the expansion's), so this stays a tuning aid.
+        // hangs off.  The staging traffic is a small part of the expansion's, so the plain allocation is the default and
+        // placement stays a tuning aid.
         int node = -1;
         if (const char *v = getenv("AIE_E2E_STAGING_NODE")) node = atoi(v);
         if (node == -2) {

@@ -1,7 +1,7 @@
 // aie_core.cuh — per-env dynamics ("step") and observation ("observe") bodies.
 //
 // Compiled two ways:
-//   * nvcc, sm_100a: NL = 32 lanes.  One warp owns one env replica whose state record lives in shared
+//   * nvcc, sm_90a: NL = 32 lanes.  One warp owns one env replica whose state record lives in shared
 //     memory.  Order-dependent sections (agent loops in np.random.permutation order, auction matching) run
 //     as warp-uniform code — every lane evaluates the same control flow from shared memory, lane 0 commits
 //     the writes — so warp collectives (MT19937 twist, redux/ballot scans of the order book) can be called

@@ -1,5 +1,5 @@
 """BatchedFoundationEnv — the Gym-style reset/step surface of the reference's BaseEnvironment
-(base/base_env.py:24-1120), over E env replicas that live on one B200.
+(base/base_env.py:24-1120), over E env replicas that live on one GPU.
 
 Differences from the reference API (all additive):
   * new kwargs `n_envs`, `device`, `seeds`, `auto_reset`, `device_reset`;

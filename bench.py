@@ -2,6 +2,7 @@
 """bench.py — agent-env-steps/sec of the gather-trade-build step (BASELINE.json).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3|c4|c5]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -11,13 +12,17 @@ collective on the step path).  Rank 0 prints ONE JSON line.
 
   value     whole-job agent-env-steps/s, inputs and outputs resident in HBM, K steps timed on the device
             (CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks)
-  sustained the same K-step region repeated until >= ~1 s of device time has been measured: median over repeats
-            (the driver's K is small; this is the number that does not depend on one 3 ms window)
   e2e       the same metric through the C-ABI host entry point with HOST (pinned) buffers: actions copied H2D and
             every observation / mask / reward / done tensor delivered to host memory inside the timed region
-  roofline  per-kernel algorithmic bytes / CUDA-event duration against MEASURED_PEAKS.json (HBM)
+  roofline  per-kernel algorithmic bytes / CUDA-event duration against MEASURED_PEAKS.json (HBM), or the H100 SXM
+            data sheet's 3.35 TB/s where that file is absent
   cpu_baseline  the CPU oracle (oracle/, a C port of the reference step) on this box's host cores
-  workloads the other BASELINE configs (c3, c4 = COVID, c5) measured the same way in the same process (headline c2 only)
+  workloads the other BASELINE configs (c3, c4 = COVID, c5) measured the same way in the same process (headline c2 only),
+            K timed steps each
+
+--dump-outputs DIR writes what the headline workload's timed path computed in its last timed step (observations, masks,
+rewards, done flags and the next actions, i.e. the tensors a caller of the step receives) as DIR/<name>.npy.  The inputs
+are seeded, so two builds run with the same arguments can be compared output for output.
 
 Episode phases are staggered before anything is timed (replica e starts at t = e*T/E and one full episode of steps is
 run untimed), so every timed window sees the whole episode distribution - full order books, houses, tax days and the
@@ -42,25 +47,25 @@ METRIC = "agent-env-steps/sec gather-trade-build"
 UNIT = "agent-env-steps/s"
 
 WORKLOADS = {
-    # BASELINE.json configs[1]: gather-trade-build, 4 agents, 25x25, 8192 env replicas per B200
-    "c2": dict(cfg="c1_tutorial", envs_per_gpu=8192, agents=4, world=[25, 25], steps=None,
+    # BASELINE.json configs[1]: gather-trade-build, 4 agents, 25x25, 8192 env replicas per GPU
+    "c2": dict(cfg="c1_tutorial", envs_per_gpu=8192, agents=4, world=[25, 25],
                desc="gather-trade-build (layout_from_file/simple_wood_and_stone: Build+CDA+Gather), 4 agents, "
                     "25x25, 8192 env replicas per GPU, uniformly random unmasked actions",
-               l2="no explicit flush: each step rewrites 296 MB of observations (> 126 MB L2) and touches 46 MB of state"),
+               l2="no explicit flush: each step rewrites 296 MB of observations (> 50 MB L2) and touches 46 MB of state"),
     # BASELINE.json configs[2]: + PeriodicBracketTax planner, 10 agents, 40x40, 65536 envs over 8 GPUs = 8192 per GPU
-    "c3": dict(cfg="c3_paper_tax", envs_per_gpu=8192, agents=10, world=[40, 40], steps=100,
+    "c3": dict(cfg="c3_paper_tax", envs_per_gpu=8192, agents=10, world=[40, 40],
                desc="gather-trade-build + PeriodicBracketTax, 10 agents, 40x40, 8192 env replicas per GPU",
-               l2="no explicit flush: each step rewrites 390 MB of observations (> 126 MB L2) and touches 87 MB of state"),
+               l2="no explicit flush: each step rewrites 390 MB of observations (> 50 MB L2) and touches 87 MB of state"),
     # BASELINE.json configs[3]: COVID-19 scenario (51 US-state agents + federal planner), 4096 envs per GPU
-    "c4": dict(cfg="covid", envs_per_gpu=4096, agents=51, world=[1, 1], steps=540,
+    "c4": dict(cfg="covid", envs_per_gpu=4096, agents=51, world=[1, 1],
                desc="COVID-19 + economy (CovidAndEconomySimulation: ControlUSStateOpenCloseStatus + "
                     "FederalGovernmentSubsidy + VaccinationCampaign), 51 state agents + planner, 4096 env replicas per GPU",
-               l2="no explicit flush: per-step footprint 163 MB (stringency history re-read every step) > 126 MB L2"),
+               l2="no explicit flush: per-step footprint 163 MB (stringency history re-read every step) > 50 MB L2"),
     # BASELINE.json configs[4]: ContinuousDoubleAuction stress, 64 agents, 64x64, deep book, 16384 envs over 8 GPUs
-    "c5": dict(cfg="c5_full", envs_per_gpu=2048, agents=64, world=[64, 64], steps=60, device_reset="snapshot",
+    "c5": dict(cfg="c5_full", envs_per_gpu=2048, agents=64, world=[64, 64], device_reset="snapshot",
                desc="CDA stress (uniform/simple_wood_and_stone: Build+CDA(max_num_orders=50)+Gather, multi-action agents), "
                     "64 agents, 64x64, 2048 env replicas per GPU",
-               l2="no explicit flush: each step rewrites 740 MB of observations (> 126 MB L2) and touches 126 MB of state"),
+               l2="no explicit flush: each step rewrites 740 MB of observations (> 50 MB L2) and touches 126 MB of state"),
 }
 
 
@@ -119,38 +124,14 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def committed_traffic(workload, kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the newest committed `ncu --set full`
-    capture of this workload (profiles/r*_ncu_full_<kernel>[_<workload>]_raw.csv); None when there is none."""
-    import csv
-    import glob
-    pats = ["r*_ncu_full_%s_%s_raw.csv" % (kernel, workload)]
-    if workload == "c2":
-        pats.append("r*_ncu_full_%s_raw.csv" % kernel)
-    found = sorted(sum((glob.glob(os.path.join(ROOT, "profiles", p)) for p in pats), []),
-                   key=lambda p: os.path.basename(p)[:4])  # by round tag
-    if not found:
-        return None, None
-    path = found[-1]
-    try:
-        rows = list(csv.reader(open(path)))
-        d, u = dict(zip(rows[0], rows[2])), dict(zip(rows[0], rows[1]))
-        scale = {"Mbyte": 1e6, "Kbyte": 1e3, "Gbyte": 1e9, "byte": 1.0}
-        tot = sum(float(d[k].replace(",", "")) * scale.get(u[k], 1.0) for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"))
-        return tot, os.path.relpath(path, ROOT)
-    except Exception:
-        return None, None
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler:
     """nvidia-smi clocks + throttle reasons sampled DURING the measured regions.
 
     Started before the warm-up steps (nvidia-smi takes a few hundred ms to come up) at a 20 ms period; mark_begin() /
-    mark_end() bracket, on the host clock, the K-step timed region plus its `sustained` repeats (the same loop, back to
-    back) and only samples time-stamped inside are reported."""
+    mark_end() bracket, on the host clock, the K-step timed region and only samples time-stamped inside are reported."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -205,7 +186,7 @@ class ClockSampler:
                 continue
         t0, t1 = self.t0 or 0.0, self.t1 or time.time()
         inside = [p for p in parsed if t0 <= p[0] <= t1 + 0.005]
-        window = "timed region + sustained repeats"
+        window = "timed region"
         if not inside:
             inside = [p for p in parsed if (self.t_start or 0.0) <= p[0] <= t1 + 0.03]
             window = "warm-up + timed region (measured regions shorter than the 20 ms sampling period)"
@@ -295,16 +276,6 @@ def cpu_baseline_for(key, min_seconds=6.0):
                       "(C oracle of the reference step), %.1f s" % (n_cpu, steps_cpu, threads, total)}
 
 
-def reference_numpy_note():
-    """The reference's own NumPy step cannot run on the GPU box (/root/reference is not there and its sources may not be
-    copied); its per-core rate measured in the build container is committed with the script that produced it."""
-    p = os.path.join(ROOT, "profiles", "reference_numpy_step.json")
-    try:
-        return json.load(open(p))
-    except Exception:
-        return None
-
-
 def run_reference_arm(args, rank, world):
     if rank != 0:
         return
@@ -334,10 +305,8 @@ def run_reference_arm(args, rank, world):
                                    % (n_envs, steps_run, threads, total)},
         "e2e": {"value": rate, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
-        "reference_numpy_step": reference_numpy_note(),
-        "note": "the reference is pure Python and does not exist on the GPU box; this arm times oracle/ (a C "
-                "restatement pinned to the reference by golden traces) on every host core it may use, which is far "
-                "faster than the reference's own NumPy step (see reference_numpy_step: measured in the build container)",
+        "note": "the reference is pure Python and is not part of this repository; this arm times oracle/ (a C "
+                "restatement pinned to the reference by golden traces) on every host core it may use",
         "wall_s": time.perf_counter() - t0,
     }
     print(json.dumps(line), flush=True)
@@ -376,17 +345,32 @@ class Ctx:
         self.barrier()
         return self.max_over_ranks(ev0.elapsed_time(ev1))
 
-    def sustained(self, one_step, k, first_ms, target_ms=1000.0, max_repeats=200):
-        """Repeat the K-step region until ~target_ms of device time is covered; median ms per step over the repeats."""
-        reps = int(min(max_repeats, max(2, np.ceil(target_ms / max(first_ms, 1e-3)))))
-        per = [first_ms / k]
-        for _ in range(reps - 1):
-            per.append(self.time_steps(one_step, k) / k)
-        return float(np.median(per)), len(per), float(min(per)), float(max(per))
 
 
-def measure_gtb(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20, e2e_mode="compact", e2e_threads=0):
-    """One gather-trade-build workload on this rank's GPU: value / sustained / per-kernel roofline / e2e."""
+def dump_outputs(out_dir, bufs, names, seed=0, budget=63 << 20):   # 63 MiB of data + the .npy headers: < 64 MiB
+    """--dump-outputs: the named tensors as they stand, as <out_dir>/<name>.npy.  float64 tensors stay float64; all others
+    become float32, which holds every value of these int16 / int32 / float32 tensors exactly.  The tensors are env-major:
+    when the batch holds more than `budget` bytes, a fixed seeded sample of env replicas (the same rows of every tensor, in
+    increasing order) is written instead."""
+    import torch
+    names = [n for n in names if n in bufs and bufs[n].numel() > 0]
+    width = {n: 8 if bufs[n].dtype == torch.float64 else 4 for n in names}
+    E = bufs[names[0]].shape[0]
+    n = min(E, budget // sum(bufs[nm][0].numel() * width[nm] for nm in names))
+    rows = np.arange(E) if n == E else np.sort(np.random.RandomState(seed).choice(E, n, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    for nm in names:
+        t = bufs[nm].index_select(0, torch.as_tensor(rows, device=bufs[nm].device))
+        np.save(os.path.join(out_dir, nm + ".npy"), t.to(torch.float64 if width[nm] == 8 else torch.float32).cpu().numpy())
+    return {"dir": out_dir, "env_replicas": int(n), "of": int(E), "seed": seed, "arrays": names}
+
+
+GTB_OUTPUTS = ["obs_agent_map", "obs_agent_idx", "obs_agent_flat", "mask_agent", "obs_planner_map", "obs_planner_idx",
+               "obs_planner_flat", "obs_planner_agents", "mask_planner", "obs_time", "reward", "done"]
+
+
+def measure_gtb(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20, e2e_mode="compact", e2e_threads=0, dump=None):
+    """One gather-trade-build workload on this rank's GPU: value / per-kernel roofline / e2e."""
     import ctypes as C
 
     torch, args, rank, world, dev = ctx.torch, ctx.args, ctx.rank, ctx.world, ctx.dev
@@ -432,10 +416,11 @@ def measure_gtb(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20, e2e_mode="c
         clocks.mark_begin()
     ms_total = ctx.time_steps(one_step, K)
     launches = st.launch_count() - launches0
-    sus_ms, sus_n, sus_min, sus_max = ctx.sustained(one_step, K, ms_total)
     if clocks:
         clocks.mark_end()
     value = world * E * A * K / (ms_total * 1e-3)
+    # the fused step also leaves the next step's actions behind: they are part of what the timed path computed
+    dumped = dump_outputs(dump, st.buf, GTB_OUTPUTS + ["actions_agent", "actions_planner"]) if dump else None
 
     # ---- per-kernel durations (separate pass, CUDA events between the kernels, same stream) ----
     n_prof = 50
@@ -477,24 +462,21 @@ def measure_gtb(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20, e2e_mode="c
         k["achieved_gbs"] = k["alg_bytes_per_launch"] / (k["ms"] * 1e-3) / 1e9
         k["frac"] = k["achieved_gbs"] / peak
     dom = "aie_step_kernel"
-    traffic, traffic_src = committed_traffic(key, dom)
     survey_bytes = step_bytes - 2 * d.state_bytes + 2 * lean_state + obs_bytes
     roofline = {"bound": "hbm", "kernel": dom, "achieved": kernels[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
-                "frac": kernels[dom]["frac"], "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
-                "alg_bytes_per_env_step": step_bytes + obs_bytes,
+                "frac": kernels[dom]["frac"], "peak_source": peak_src, "alg_bytes_per_env_step": step_bytes + obs_bytes,
                 "frac_on_survey_8d_bytes": {"alg_bytes_per_env_step": survey_bytes,
                                             "frac": E * survey_bytes / (kernels[dom]["ms"] * 1e-3) / 1e9 / peak,
                                             "what": "SURVEY §8(d)'s accounting: record without the 2.5 KB MT19937 key and the "
                                                     "episode statistics (both travel in and out with the record here)"},
                 "whole_step": {"alg_bytes_per_env_step": d.algorithmic_bytes_per_env_step,
-                               "achieved": d.algorithmic_bytes_per_env_step * E / (sus_ms * 1e-3) / 1e9,
-                               "frac": d.algorithmic_bytes_per_env_step * E / (sus_ms * 1e-3) / 1e9 / peak},
+                               "achieved": d.algorithmic_bytes_per_env_step * E * K / (ms_total * 1e-3) / 1e9,
+                               "frac": d.algorithmic_bytes_per_env_step * E * K / (ms_total * 1e-3) / 1e9 / peak},
                 "kernels": kernels}
 
     # ---- e2e through the host entry point with pinned HOST buffers ----
     out_host, out_ptrs, d2h = {}, {}, 0
-    for nm in ["obs_agent_map", "obs_agent_idx", "obs_agent_flat", "mask_agent", "obs_planner_map", "obs_planner_idx",
-               "obs_planner_flat", "obs_planner_agents", "mask_planner", "obs_time", "reward", "done"]:
+    for nm in GTB_OUTPUTS:
         if nm in st.buf:
             # pinned host tensors from the package's allocator: blocks of replicas (one transfer slice each) on alternating
             # NUMA nodes, which is what the node-pinned expansion threads of aie_step_host_compact are matched to: every
@@ -554,14 +536,13 @@ def measure_gtb(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20, e2e_mode="c
                         "(same bytes in the host tensors as the plain path)")
     res = {
         "value": value, "ms_per_step": ms_total / K, "steps": K, "warmup": W,
-        "sustained": {"ms_per_step": sus_ms, "value": world * E * A / (sus_ms * 1e-3), "repeats": sus_n,
-                      "min_ms_per_step": sus_min, "max_ms_per_step": sus_max,
-                      "what": "median over repeats of the K-step timed region (same loop, same synchronisation)"},
         "config": dict(workload_config(key, E), parallelism="env replicas sharded over %d GPU(s), no collective on "
                        "the step path" % world, setup_s=t_setup, device_reset=("reference-exact (reset_mode 1)"
                        if env.spec.get("reset_mode", 0) == 1 else "snapshot restore (reset_mode 0)")),
         "e2e": e2e, "gpu_launches": launches, "roofline": roofline, "dtype": "i32+f64", "n_agents": A,
     }
+    if dumped:
+        res["dump_outputs"] = dumped
     if with_cpu:
         res["cpu_baseline"] = cpu_baseline_for(key)
     del env, st, out_host, act_a, act_p
@@ -590,7 +571,7 @@ def measure_gtb(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20, e2e_mode="c
     return res
 
 
-def measure_covid(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20):
+def measure_covid(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20, dump=None):
     """BASELINE config 4: one fused kernel per step (+ the random-policy sampler)."""
     torch, args, rank, world, dev = ctx.torch, ctx.args, ctx.rank, ctx.world, ctx.dev
     from ai_economist_b200 import foundation
@@ -616,10 +597,12 @@ def measure_covid(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20):
         clocks.mark_begin()
     ms_total = ctx.time_steps(one_step, K)
     launches = st.launch_count() - l0
-    sus_ms, sus_n, sus_min, sus_max = ctx.sustained(one_step, K, ms_total, max_repeats=20)
     if clocks:
         clocks.mark_end()
     value = world * E * S * K / (ms_total * 1e-3)
+    names = ["obs_agent_state", "obs_postsubsidy", "obs_lagged_stringency", "obs_policy_indicators", "obs_scalars",
+             "mask_agent", "mask_planner", "reward_agent", "reward_planner", "done"]
+    dumped = dump_outputs(dump, st.buf, names + ["actions_agent", "actions_planner"]) if dump else None
     # per-kernel durations: the cost of the history scan depends on how many stringency changes the window holds, so
     # the event-separated pass replays the SAME stretch of the episode as the timed region (reset, same warm-up)
     env.reset()
@@ -643,10 +626,7 @@ def measure_covid(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20):
         k["achieved_gbs"] = k["alg_bytes_per_launch"] / (k["ms"] * 1e-3) / 1e9
         k["frac"] = k["achieved_gbs"] / peak
     dom = "aie_covid_step_kernel"
-    traffic, traffic_src = committed_traffic(key, dom)
     # e2e: pinned host actions in, all outputs back
-    names = ["obs_agent_state", "obs_postsubsidy", "obs_lagged_stringency", "obs_policy_indicators", "obs_scalars",
-             "mask_agent", "mask_planner", "reward_agent", "reward_planner", "done"]
     host = {n: torch.empty(st.buf[n].shape, dtype=st.buf[n].dtype, pin_memory=True) for n in names}
     act_a = torch.zeros((E, S), dtype=torch.int32, pin_memory=True)
     act_p = torch.zeros((E,), dtype=torch.int32, pin_memory=True)
@@ -670,19 +650,16 @@ def measure_covid(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20):
     e2e_value = world * E * S * n_e2e / ctx.max_over_ranks(e2e_s)
     res = {
         "value": value, "ms_per_step": ms_total / K, "steps": K, "warmup": W,
-        "sustained": {"ms_per_step": sus_ms, "value": world * E * S / (sus_ms * 1e-3), "repeats": sus_n,
-                      "min_ms_per_step": sus_min, "max_ms_per_step": sus_max,
-                      "what": "median over repeats of the K-step timed region"},
         "config": dict(workload_config(key, E), parallelism="env replicas sharded over %d GPU(s), no collective on the "
-                       "step path" % world, episode_phase="lock-step (deterministic scenario); the timed region covers "
-                       "the episode from the warm-up on, K = 540 is one whole episode"),
+                       "step path" % world, episode_phase="lock-step (deterministic scenario, 540-step episodes); the timed "
+                       "region covers K steps from the warm-up on, auto-resets included"),
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": E * (S + 1) * 4, "d2h_bytes_per_step": d2h,
                 "steps": n_e2e, "what": "pinned host actions -> device, step, every observation/mask/reward/done tensor "
                                         "back to pinned host"},
         "gpu_launches": launches, "dtype": "f32+f64", "n_agents": S,
+        **({"dump_outputs": dumped} if dumped else {}),
         "roofline": {"bound": "hbm", "kernel": dom, "achieved": kernels[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
-                     "frac": kernels[dom]["frac"], "traffic": traffic, "traffic_source": traffic_src,
-                     "peak_source": peak_src, "alg_bytes_per_env_step": step_bytes, "kernels": kernels},
+                     "frac": kernels[dom]["frac"], "peak_source": peak_src, "alg_bytes_per_env_step": step_bytes, "kernels": kernels},
     }
     if with_cpu:
         res["cpu_baseline"] = cpu_baseline_for(key)
@@ -696,10 +673,10 @@ def measure_covid(ctx, key, K, W, with_cpu, clocks=None, e2e_steps=20):
 
 def reference_cuda_leg(ctx, params, E, K, ours_ms_per_step, ours_step_kernel_ms):
     """Baseline leg for config 4: the reference's OWN CUDA kernels (covid19_env_step.cu / covid19_components_step.cu,
-    compiled for sm_100a from /root/reference into oracle/_ref/ by oracle/build_ref_covid.py) on the same GPU, same
+    compiled for sm_90a from the reference's sources into oracle/_ref/ by oracle/build_ref_covid.py) on the same GPU, same
     number of replicas, launched the way the reference's wrapper launches them (grid = envs, block = 52, five launches
     per step).  Like cpu_baseline this is a reported baseline, never the thing shipped; None when the library was not
-    built (no /root/reference at build time).  Its kernels' cost does not depend on the actions (they rewrite the whole
+    built (no reference sources at build time).  Its kernels' cost does not depend on the actions (they rewrite the whole
     convolution signal every step), so a fixed action tensor is stepped and its reset copy is left out (in its favour)."""
     try:
         from oracle import build_ref_covid
@@ -719,7 +696,7 @@ def reference_cuda_leg(ctx, params, E, K, ours_ms_per_step, ours_step_kernel_ms)
         out = {"ms_per_step": ms / K, "value": ctx.world * E * 51 * K / (ms * 1e-3), "unit": UNIT, "steps": K, "envs_per_gpu": E,
                "launches_per_step": ref.launches_per_step(), "speedup_whole_step": (ms / K) / ours_ms_per_step,
                "speedup_step_kernel_only": (ms / K) / ours_step_kernel_ms,
-               "what": "reference CUDA kernels (sm_100a build of the unmodified sources, nvcc -O3) on this GPU: "
+               "what": "reference CUDA kernels (sm_90a build of the unmodified sources, nvcc -O3) on this GPU: "
                        "CudaControlUSStateOpenCloseStatusStep, CudaFederalGovernmentSubsidyStep, CudaVaccinationCampaignStep, "
                        "CudaCovidAndEconomySimulationStep, CudaComputeReward; speedup = its ms/step over ours (sampler + step)"}
         del ref
@@ -733,9 +710,8 @@ def compact(res):
     """What a sub-workload contributes to the headline line's `workloads` object."""
     r = res["roofline"]
     return {"value": res["value"], "ms_per_step": res["ms_per_step"], "steps": res["steps"],
-            "sustained": {k: res["sustained"][k] for k in ("ms_per_step", "value", "repeats")},
-            "roofline": {"kernel": r["kernel"], "frac": r["frac"], "achieved": r["achieved"], "traffic": r["traffic"],
-                         "traffic_source": r.get("traffic_source"), "alg_bytes_per_env_step": r["alg_bytes_per_env_step"],
+            "roofline": {"kernel": r["kernel"], "frac": r["frac"], "achieved": r["achieved"],
+                         "alg_bytes_per_env_step": r["alg_bytes_per_env_step"],
                          "kernel_ms": {k: v["ms"] for k, v in r["kernels"].items()}},
             "e2e": res["e2e"], "gpu_launches": res["gpu_launches"], "n_agents": res["n_agents"],
             "envs_per_gpu": res["config"]["envs_per_gpu"], "device_reset": res["config"].get("device_reset"),
@@ -762,6 +738,8 @@ def main():
     ap.add_argument("--preroll", type=int, default=None, help="untimed steps after staggering the episode phases (default: one episode)")
     ap.add_argument("--no-extra-workloads", action="store_true",
                     help="headline workload only (skip the c3/c4/c5 entries of `workloads`)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline workload's outputs of its last timed step as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -787,10 +765,10 @@ def main():
         clocks.start()
     fn = measure_covid if key == "c4" else measure_gtb
     if args.e2e_threads == 0:   # expansion threads of the e2e leg: this rank's share of half the host's hardware threads
-        # (one per physical core: the expansion is bound by the memory controllers, 48 - 64 threads are as fast as 96 on the
-        # 2 x 32-core B200 host and burn half the CPU time, profiles/r02z_e2e_transfer_knobs.txt section 7)
+        # (one per physical core: the expansion is bound by the memory controllers, and hyper-threads add CPU time, not speed)
         args.e2e_threads = max(8, host_cores() // (2 * max(1, world)))
     kw = {} if key == "c4" else dict(e2e_mode=args.e2e_mode, e2e_threads=args.e2e_threads)
+    kw["dump"] = args.dump_outputs if rank == 0 else None
     res = fn(ctx, key, args.steps, args.warmup, with_cpu, clocks=clocks, e2e_steps=args.e2e_steps, **kw)
     clk = clocks.stop() if clocks else None
     extra = {}
@@ -799,7 +777,7 @@ def main():
             f2 = measure_covid if k2 == "c4" else measure_gtb
             kw2 = {} if k2 == "c4" else dict(e2e_mode=args.e2e_mode, e2e_threads=args.e2e_threads)
             try:
-                extra[k2] = compact(f2(ctx, k2, WORKLOADS[k2]["steps"], max(3, min(args.warmup, 20)), False, e2e_steps=10, **kw2))
+                extra[k2] = compact(f2(ctx, k2, args.steps, max(3, min(args.warmup, 20)), False, e2e_steps=10, **kw2))
             except Exception as ex:   # the headline line must survive a failing extra workload (all ranks fail alike)
                 extra[k2] = {"error": "%s: %s" % (type(ex).__name__, ex)}
     if rank != 0:
@@ -810,16 +788,17 @@ def main():
         "metric": METRIC if key != "c4" else METRIC.replace("gather-trade-build", "covid19"),
         "value": res["value"], "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": res["ms_per_step"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": res["dtype"], "data": "synthetic", "config": res["config"], "clocks": clk, "sustained": res["sustained"],
+        "dtype": res["dtype"], "data": "synthetic", "config": res["config"], "clocks": clk,
         "e2e": res["e2e"], "gpu_launches": res["gpu_launches"], "roofline": res["roofline"],
     }
     if "cpu_baseline" in res:
         line["cpu_baseline"] = res["cpu_baseline"]
-        line["reference_numpy_step"] = reference_numpy_note()
     if "vs_reference_cuda" in res:
         line["vs_reference_cuda"] = res["vs_reference_cuda"]
     if extra:
         line["workloads"] = extra
+    if "dump_outputs" in res:
+        line["dump_outputs"] = res["dump_outputs"]
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()

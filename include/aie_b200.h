@@ -1,5 +1,5 @@
 /*
- * aie_b200.h — C-ABI of the B200-native batched Foundation environment stepper.
+ * aie_b200.h — C-ABI of the H100-native (sm_90a) batched Foundation environment stepper.
  *
  * Drop-in boundary for the reference's per-timestep hot path
  *   BaseEnvironment.step()                     ai_economist/foundation/base/base_env.py:929-1032

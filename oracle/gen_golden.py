@@ -52,6 +52,14 @@ PLAN = [
     ("multi_zone_reset", 1001, 90, 8),
 ]
 
+# tests/test_oracle_vs_reference.py: other seeds and lengths, full observations at every step
+PLAN_LIVE = [
+    ("c1_tutorial", 31, 150, 1),
+    ("c3_short_period", 32, 120, 1),
+    ("c5_small", 33, 40, 1),
+    ("ref_unit_test", 34, 60, 1),
+]
+
 EXACT_OBS = ["a_map", "a_idx", "a_mask", "p_map", "p_idx", "p_mask"]
 FLOAT_OBS = ["a_flat", "p_flat", "p_agents", "time"]
 STEP_STATE = ["loc", "inv", "esc", "coin", "esc_coin", "labor", "n_orders", "tax_pos", "rate_idx",
@@ -62,7 +70,7 @@ def crc(a):
     return zlib.crc32(np.ascontiguousarray(a).tobytes()) & 0xFFFFFFFF
 
 
-def generate(cfg_name, seed, steps, full_every):
+def generate(cfg_name, seed, steps, full_every, out_dir=None):
     f = rh.load_reference_foundation()
     cfg = dict(CONFIGS[cfg_name])
     env = f.make_env_instance(**cfg)
@@ -128,7 +136,8 @@ def generate(cfg_name, seed, steps, full_every):
             if k in ("a_map", "p_map"):
                 arr = arr.astype(np.uint8)  # 0/1-valued float32 planes: stored as u8, compared after cast
             out["full_" + k] = arr
-    out_dir = OUT + "_reset" if cfg_name.endswith("_reset") else OUT   # multi-episode traces live apart
+    if out_dir is None:
+        out_dir = OUT + "_reset" if cfg_name.endswith("_reset") else OUT   # multi-episode traces live apart
     os.makedirs(out_dir, exist_ok=True)
     path = os.path.join(out_dir, "%s_seed%d.npz" % (cfg_name, seed))
     np.savez_compressed(path, **out)
@@ -141,3 +150,6 @@ if __name__ == "__main__":
     for item in PLAN:
         if not only or item[0] in only:
             generate(*item)
+    for item in PLAN_LIVE:
+        if not only or item[0] in only:
+            generate(*item, out_dir=os.path.join(OUT, "live"))

@@ -1,11 +1,11 @@
 // TEST / BASELINE INFRASTRUCTURE - not part of the product, never loaded by ai_economist_b200/.
 //
 // Host-side launcher for the REFERENCE's own COVID-19 CUDA kernels, so that they can be run and timed on the same
-// B200 as aie_covid_step_kernel (BASELINE.md config 4: "additionally the reference's CUDA kernels if they can be built
-// on the GPU box").  The kernels are NOT copied: this file #includes the reference's build unit where it lies under
-// /root/reference at compile time (REF_COVID_BUILD_CU, passed by oracle/build_ref_covid.py), and the output goes to
+// GPU as aie_covid_step_kernel (BASELINE.md config 4: the reference's CUDA kernels as an additional bar where they can be
+// built).  The kernels are NOT copied: this file #includes the reference's build unit where it lies in a
+// reference checkout at compile time (REF_COVID_BUILD_CU, passed by oracle/build_ref_covid.py), and the output goes to
 // oracle/_ref/ (git-ignored).  What is written here is only the launch sequence, which in the reference lives in
-// Python on top of WarpDrive / PyCUDA (absent from this image):
+// Python on top of WarpDrive / PyCUDA (not a dependency of this project):
 //   components/covid19_components.py:145-172, 355-383, 587-608   component_step() GPU branches, in component order
 //   scenarios/covid19/covid19_env.py:650-705                      scenario_step() GPU branch (includes observations)
 //   scenarios/covid19/covid19_env.py:995-1040                     compute_reward() GPU branch

@@ -13,6 +13,8 @@ import types
 
 import numpy as np
 
+from oracle import ref_tape
+
 REFERENCE_ROOT = os.environ.get("AIE_REFERENCE_ROOT", "/root/reference")
 
 
@@ -24,7 +26,15 @@ _foundation = None
 
 
 def load_reference_foundation():
-    """Import `ai_economist.foundation` from the read-only reference tree."""
+    """Import `ai_economist.foundation` from the read-only reference tree.  Inside a test run under
+    oracle.ref_tape.taped this is a recording proxy of it, or its replay where the reference tree is absent."""
+    from oracle import ref_tape
+    if ref_tape.active() is not None:
+        return ref_tape.wrap_foundation(_import_foundation() if reference_available() else None)
+    return _import_foundation()
+
+
+def _import_foundation():
     global _foundation
     if _foundation is not None:
         return _foundation
@@ -58,6 +68,7 @@ def load_reference_foundation():
 COMPONENT_NAMES = ["Build", "ContinuousDoubleAuction", "Gather", "PeriodicBracketTax", "WealthRedistribution"]
 
 
+@ref_tape.recorded
 def spec_from_reference_env(env):
     """Read a flat config dict (the oracle's orc_config fields) off a constructed reference env."""
     comps = [c.name for c in env._components]
@@ -121,13 +132,14 @@ def spec_from_reference_env(env):
     return spec
 
 
+@ref_tape.recorded
 def state_from_reference_env(env):
     """Post-reset host snapshot (call right after env.reset())."""
     maps = env.world.maps
     A = env.n_agents
     H, W = env.world_size
     water = maps.get("Water") if "Water" in maps.keys() else np.zeros((H, W))
-    key = np.random.get_state()
+    key = ref_tape.global_stream_state()
     st = dict(
         stone=(maps.get("Stone") > 0).astype(np.uint8), wood=(maps.get("Wood") > 0).astype(np.uint8),
         stone_src=(maps.get("StoneSourceBlock") > 0).astype(np.uint8),
@@ -150,6 +162,7 @@ def state_from_reference_env(env):
     return st
 
 
+@ref_tape.recorded
 def obs_arrays_from_reference(env, obs, rew=None, done=None):
     """Reference obs dict (flatten_observations=True, flatten_masks=True) -> oracle-layout arrays."""
     A = env.n_agents
@@ -174,6 +187,7 @@ def obs_arrays_from_reference(env, obs, rew=None, done=None):
     return out
 
 
+@ref_tape.recorded
 def state_arrays_from_reference(env):
     """Full mid-episode state of the reference env in the oracle's orc_get_state layout."""
     maps = env.world.maps
@@ -185,7 +199,7 @@ def state_arrays_from_reference(env):
             | ((maps.get("WoodSourceBlock") > 0).astype(np.uint8) << 3)
             | ((water > 0).astype(np.uint8) << 4) | ((maps.get("House") > 0).astype(np.uint8) << 5))
     ag = env.world.agents
-    key = np.random.get_state()
+    key = ref_tape.global_stream_state()
     out = dict(
         cell=cell, owner=maps.get("House", owner=True).astype(np.int8),
         loc=np.array([[int(a.loc[0]), int(a.loc[1])] for a in ag], np.int16),

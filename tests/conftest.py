@@ -9,16 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
-    config.addinivalue_line("markers", "reference: needs the read-only reference tree at /root/reference")
-
-
-# GPU cases that have not run on a B200 yet go here (substring of the node id): they are ordered last, so that with `-x`
-# a surprise there cannot mask the cases that are known to pass on the hardware.  Everything else has run on a B200
-# (profiles/r02z_pytest_gpu.log: 141 passed).  saez_annealed: the Saez model under a tax_annealing_schedule was added after
-# the round's last GPU minute; it is green on the host emulation of the same device source and changes only the `EXT`
-# kernel instantiations (the SASS of every other kernel is byte-identical to the measured build).
-NOT_YET_RUN_ON_B200 = ("saez_annealed",)
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: the library is built for sm_90a)")
+    config.addinivalue_line("markers", "reference: compares with the reference: live where a checkout exists, else its recorded tape")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -28,7 +20,3 @@ def pytest_collection_modifyitems(config, items):
     for item in items:
         if "gpu" in item.keywords and not has_gpu:
             item.add_marker(pytest.mark.skip(reason="no CUDA device"))
-    late = [i for i in items if "gpu" in i.keywords and any(n in i.nodeid for n in NOT_YET_RUN_ON_B200)]
-    if late:
-        ids = {id(i) for i in late}
-        items[:] = [i for i in items if id(i) not in ids] + late

@@ -4,7 +4,7 @@
 // (-DAIE_EMU, NL = 1: warp collectives become identities) behind the very same C-ABI implementation
 // (aie_abi.inl) and check it against the golden traces and the C oracle.  This validates the algorithmic
 // content of the kernels (not their warp synchronisation, which the `-m gpu` tests and compute-sanitizer
-// cover on the B200).  The product never builds, ships or loads this file: ai_economist_b200/_lib.py only
+// cover on the GPU).  The product never builds, ships or loads this file: ai_economist_b200/_lib.py only
 // opens libaie_b200.so (CUDA) and raises if it is missing.
 #define AIE_EMU 1
 #include <stdint.h>

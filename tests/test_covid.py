@@ -16,6 +16,7 @@ import pytest
 
 from ai_economist_b200.foundation.covid19 import build_covid_params
 from oracle.covid_oracle import CovidOracleEnv
+from oracle.ref_tape import taped
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden_covid", "covid_seed3.npz")
 OBS_KEYS = ["agent_state", "postsubsidy", "lagged", "policy_ind", "scalars", "mask_a", "mask_p"]
@@ -240,8 +241,8 @@ def test_covid_env_api_through_make_env_instance():
 
 
 @pytest.mark.reference
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference tree not present")
 @pytest.mark.parametrize("variant", range(4))
+@taped
 def test_covid_observe_rate_matches_live_reference(variant):
     """VaccinationCampaign(observe_rate=True) (covid19_components.py:629-661): `next_vaccination_rate` for agents and planner is
     a function of the timestep alone; the facade serves it by table lookup after every step / reset.  Variants: deliveries from

@@ -11,6 +11,7 @@ import pytest
 
 from oracle import configs
 from oracle import ref_harness as rh
+from oracle.ref_tape import taped
 
 EDGE = sorted(configs.EDGE_CONFIGS)
 
@@ -47,8 +48,8 @@ def test_emulated_device_code_matches_oracle_on_edge_config(cfg):
 
 
 @pytest.mark.reference
-@pytest.mark.skipif(not rh.reference_available(), reason="reference tree not present")
 @pytest.mark.parametrize("cfg", EDGE)
+@taped
 def test_oracle_and_host_reset_track_live_reference_on_edge_config(cfg):
     from oracle.validate_vs_reference import run
     _all_configs()

@@ -2,8 +2,7 @@
 
 The fuzzers draw configurations from the whole supported option space (scenario families, component subsets and orders,
 both action modes, tax models incl. annealing, WealthRedistribution, view radius, full observability, regen halfwidths,
-social welfare functions, skill distributions).  Unbounded runs are a tool (`python tools/fuzz_*.py N SEED`, logs under
-profiles/); here every fuzzer contributes N_CASES configurations drawn from a fixed seed, one test case each:
+social welfare functions, skill distributions).  Unbounded runs are a tool (`python tools/fuzz_*.py N SEED`); here every fuzzer contributes N_CASES configurations drawn from a fixed seed, one test case each:
 
   * emu vs oracle            CPU, always            the device source (1-lane emulation) against the C oracle
   * cuda vs oracle           -m gpu                 the same configurations on the CUDA build (through the C-ABI)
@@ -15,7 +14,8 @@ profiles/); here every fuzzer contributes N_CASES configurations drawn from a fi
   * Saez hybrid vs reference -m reference           the Saez tax model (device / host), with and without tax annealing
   * COVID vs reference       -m reference           COVID device code (scan and change list) under parameter variants
 
-`-m reference` cases need /root/reference (build container) and are skipped elsewhere.
+`-m reference` cases run against the live reference where a checkout is present, and against what it returned there
+(tests/golden/reference_tapes/, oracle/ref_tape.py) everywhere else.
 """
 import os
 import sys
@@ -27,10 +27,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import fuzz_emu_vs_oracle as fz  # noqa: E402
-from oracle import ref_harness as rh  # noqa: E402
+from oracle.ref_tape import taped  # noqa: E402
 
 N_CASES = 20
-needs_reference = pytest.mark.skipif(not rh.reference_available(), reason="reference tree not present")
 
 
 def _configs(seed, n=N_CASES, draw=None):
@@ -77,9 +76,9 @@ def test_fuzz_cuda_matches_oracle(i):
     bu.run_pair(env, orc, min(60, kw["episode_length"]), np.random.RandomState(1 + i), check_every=15)
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(N_CASES))
+@taped
 def test_fuzz_oracle_matches_live_reference(i):
     from oracle import configs
     from oracle.validate_vs_reference import run
@@ -93,9 +92,9 @@ def test_fuzz_oracle_matches_live_reference(i):
     assert ok
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(N_CASES))
+@taped
 def test_fuzz_device_reset_matches_live_reference(i):
     import fuzz_device_reset_vs_reference as fr
 
@@ -103,9 +102,9 @@ def test_fuzz_device_reset_matches_live_reference(i):
     fr.run_one(cfg, seed=500 + i, episodes=3)
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(N_CASES))
+@taped
 def test_fuzz_dynamic_layout_device_reset_matches_live_reference(i):
     """uniform / quadrant: the device generates a new clumped layout at every auto-reset (rand thinning, randn + convolve2d
     growth, coverage retries, checkering, water lines) and must land on the reference's maps, placements and stream."""
@@ -118,9 +117,9 @@ def test_fuzz_dynamic_layout_device_reset_matches_live_reference(i):
         pytest.skip(repr(ex))
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(10))
+@taped
 def test_fuzz_multi_zone_device_reset_matches_live_reference(i, monkeypatch):
     """multi_zone: np.random.shuffle of the region -> zone-type vector on the device before every layout."""
     import fuzz_device_reset_vs_reference as fr
@@ -135,9 +134,9 @@ def test_fuzz_multi_zone_device_reset_matches_live_reference(i, monkeypatch):
         pytest.skip(repr(ex))   # the reference refusing its own configuration
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(10))
+@taped
 def test_fuzz_saez_hybrid_matches_live_reference(i):
     """PeriodicBracketTax(tax_model="saez"): warm-up draws on the device, buffer / regression / formula on the host, rates in
     force and observed across resets - random bracket layouts, weights, fixed elasticities, rate bounds, with and without a
@@ -148,9 +147,9 @@ def test_fuzz_saez_hybrid_matches_live_reference(i):
     fr.run_one(cfg, seed=800 + i, episodes=fr.saez_episodes(cfg))
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(N_CASES))
+@taped
 def test_fuzz_reference_api_matches_live_reference(i):
     import fuzz_reference_api_vs_reference as fa
 
@@ -158,9 +157,9 @@ def test_fuzz_reference_api_matches_live_reference(i):
     _skip_unsupported(fa.run_one, name, kw, seed=700 + i)
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(N_CASES))
+@taped
 def test_fuzz_one_step_economy_matches_live_reference(i):
     """SimpleLabor + one-step-economy (components/simple_labor.py, scenarios/one_step_economy): observations, masks, rewards,
     numpy stream and finished-episode metrics across auto-resets, random reward types / tax settings / populations."""
@@ -170,9 +169,9 @@ def test_fuzz_one_step_economy_matches_live_reference(i):
     fo.run_one(cfg, seed=300 + i, episodes=3)
 
 
-@needs_reference
 @pytest.mark.reference
 @pytest.mark.parametrize("i", range(8))
+@taped
 def test_fuzz_covid_matches_live_reference(i):
     import fuzz_covid_vs_reference as fc
 

@@ -1,4 +1,4 @@
-"""GPU (B200): the CUDA product, called through the C-ABI, against (1) the golden traces recorded from the
+"""GPU: the CUDA product, called through the C-ABI, against (1) the golden traces recorded from the
 unmodified reference and (2) the C oracle on identical seeds + action sequences.
 
 Tolerances (BASELINE.json north_star): bit-exact for grid / inventory / index / mask / RNG state; <= 1e-6

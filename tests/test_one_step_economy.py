@@ -16,6 +16,7 @@ import numpy as np
 import pytest
 
 from ai_economist_b200 import foundation
+from oracle.ref_tape import taped
 
 FILES = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden_one_step", "*.npz")))
 
@@ -90,12 +91,11 @@ def test_one_step_economy_rejects_what_the_reference_rejects():
 
 
 @pytest.mark.reference
+@taped
 def test_reference_api_facade_runs_the_one_step_economy_like_the_reference():
     """reference_api=True: the reference's single-env interface (nested dicts, named fields) over replica 0, side by side with
     the live reference through three episodes: observations, rewards, done, metrics."""
     from oracle import ref_harness as rh
-    if not rh.reference_available():
-        pytest.skip("reference tree not present")
     from tests.emu.emu_stepper import emu_factory
     cfg = dict(components=[("SimpleLabor", dict(mask_first_step=True, payment_max_skill_multiplier=3)),
                            ("PeriodicBracketTax", dict(bracket_spacing="us-federal", period=2, tax_model="model_wrapper", rate_disc=0.05))],

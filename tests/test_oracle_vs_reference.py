@@ -1,16 +1,22 @@
-"""CPU, build-container only: the C oracle against the *live* imported reference (skipped where
-/root/reference is absent, e.g. on the GPU box).  Shorter than the golden traces; different seeds."""
+"""CPU: the C oracle against the reference on seeds and lengths other than the golden traces', with the full observations
+compared at every step: against traces recorded from the unmodified reference (tests/golden/live/, written by
+oracle/gen_golden.py), and in addition against the live imported reference wherever a reference checkout is present."""
+import os
+
 import pytest
 
 from oracle import ref_harness as rh
+from tests import golden_utils as gu
+from tests.test_oracle_golden import OracleStepper
 
-pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="reference tree not present")
+LIVE_DIR = os.path.join(gu.GOLDEN_DIR, "live")
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize("cfg,seed,steps", [
     ("c1_tutorial", 31, 150), ("c3_short_period", 32, 120), ("c5_small", 33, 40), ("ref_unit_test", 34, 60),
 ])
 def test_oracle_tracks_live_reference(cfg, seed, steps):
-    from oracle.validate_vs_reference import run
-    assert run(cfg, seed, steps, verbose=False)
+    assert gu.replay(os.path.join(LIVE_DIR, "%s_seed%d.npz" % (cfg, seed)), OracleStepper) == steps
+    if rh.reference_available():
+        from oracle.validate_vs_reference import run
+        assert run(cfg, seed, steps, verbose=False)

@@ -7,6 +7,7 @@ import pytest
 from ai_economist_b200 import foundation
 from oracle import ref_harness as rh
 from tests.emu.emu_stepper import emu_factory
+from oracle.ref_tape import taped
 
 # tutorials/economic_simulation_basic.ipynb cell 11, verbatim apart from a shorter episode
 ENV_CONFIG = {
@@ -70,13 +71,13 @@ def test_tutorial_loop_runs_unchanged_on_the_reference_api():
 
 
 @pytest.mark.reference
-@pytest.mark.skipif(not rh.reference_available(), reason="reference tree not present")
 @pytest.mark.parametrize("flags", [dict(flatten_observations=False, flatten_masks=True),
                                    dict(flatten_observations=True, flatten_masks=True),
                                    # schedules that live across resets: the "auto" warm-up integrator, completions
                                    dict(energy_warmup_constant=3, energy_warmup_method="auto", episode_length=30),
                                    dict(energy_warmup_constant=2, energy_warmup_method="decay", episode_length=30)],
                          ids=["named_fields", "flat", "auto_warmup", "decay_warmup"])
+@taped
 def test_reference_api_tracks_the_live_reference(flags):
     """Same config, same seed, same caller code on both: identical observation structure and values, two episodes."""
     cfg = dict(ENV_CONFIG)
@@ -168,7 +169,7 @@ def test_replay_log_reproduces_an_episode():
 
 
 @pytest.mark.reference
-@pytest.mark.skipif(not rh.reference_available(), reason="reference tree not present")
+@taped
 def test_a_replay_log_recorded_by_the_reference_replays_here():
     """Cross-implementation replay: the unmodified reference plays an episode and hands over its replay log; replaying
     that log through the facade ends in the reference's final state and metrics (and the other way round)."""

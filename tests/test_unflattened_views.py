@@ -7,6 +7,7 @@ from ai_economist_b200 import foundation
 from oracle import ref_harness as rh
 from oracle.configs import CONFIGS
 from tests.emu.emu_stepper import emu_factory
+from oracle.ref_tape import taped
 
 
 def _product(cfg, **over):
@@ -48,8 +49,8 @@ def test_named_fields_are_slices_of_the_flat_vectors(cfg):
 
 
 @pytest.mark.reference
-@pytest.mark.skipif(not rh.reference_available(), reason="reference tree not present")
 @pytest.mark.parametrize("cfg", ["c1_tutorial", "c3_short_period", "tax_us_federal", "full_obs_tax"])
+@taped
 def test_unflattened_observations_match_live_reference(cfg):
     f = rh.load_reference_foundation()
     kw = dict(CONFIGS[cfg])

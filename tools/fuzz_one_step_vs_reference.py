@@ -10,7 +10,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from ai_economist_b200 import foundation  # noqa: E402
-from oracle import ref_harness as rh  # noqa: E402
+from oracle import ref_harness as rh, ref_tape  # noqa: E402
 from tests.emu.emu_stepper import emu_factory  # noqa: E402
 
 
@@ -43,7 +43,7 @@ def reference_arrays(ref, obs):
                p_agents=(np.stack([obs["p"]["p%d" % i] for i in range(A)]).astype(np.float32) if "p0" in obs["p"]
                          else np.zeros((A, 0), np.float32)),
                time=np.asarray(obs["p"]["time"], np.float32))
-    key = np.random.get_state()
+    key = ref_tape.global_stream_state()
     out["mt_key"], out["mt_pos"] = np.array(key[1], np.uint32), int(key[2])
     ag = ref.world.agents
     out["coin"] = np.array([a.state["inventory"]["Coin"] for a in ag], np.float64)

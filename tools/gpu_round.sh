@@ -1,5 +1,5 @@
 #!/bin/bash
-# Runs on the B200 box under gpurun: parity tests, smoke, bench, ncu launch list + full captures, sanitizers.
+# Runs on the GPU machine: parity tests, smoke, bench, ncu launch list + full captures, sanitizers.
 # Everything of interest lands in gpurun_out/.   usage: bash tools/gpu_round.sh [all|test,smoke,bench,ncu,race,...]
 set -u
 mkdir -p gpurun_out

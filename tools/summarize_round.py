@@ -89,7 +89,7 @@ if os.path.exists(lp):
 
 b = json.load(open(os.path.join(OUT, "bench.json")))
 k = b["roofline"]["kernels"]
-lines = ["# Round 1 (%s) — B200 measurements, workload c2 (4 agents, 25x25, 8192 env replicas, 1 GPU)" % tag[-1], "",
+lines = ["# Round 1 (%s) — H100 measurements, workload c2 (4 agents, 25x25, 8192 env replicas, 1 GPU)" % tag[-1], "",
          "Command: `bash tools/gpu_round.sh all` under gpurun; artefacts copied by `tools/summarize_round.py %s`." % tag, "",
          "## bench.py (CUDA events, %d steps after %d warm-up)" % (b["steps"], b["warmup"]), "",
          "* value = %.3e agent-env-steps/s (%.4f ms per step of 8192 envs); e2e (all outputs to pinned host) = %.3e"
@@ -129,7 +129,7 @@ if "aie_step_kernel" in raw:
                  ", ".join("%s %.2f" % kv for kv in sorted(stall.items(), key=lambda x: -x[1])[:10]))
     tr = float(d["dram__bytes_read.sum"]) + float(d["dram__bytes_write.sum"])
     lines.append("")
-    lines.append("traffic = dram read + write = %.1f MB per launch vs %.1f MB algorithmic: no re-reads; the L2 (126 MB) absorbs part "
+    lines.append("traffic = dram read + write = %.1f MB per launch vs %.1f MB algorithmic: no re-reads; the L2 (50 MB) absorbs part "
                  "of the record write-back." % (tr, k["aie_step_kernel"]["alg_bytes_per_launch"] / 1e6))
 for f in ("racecheck.log", "memcheck.log"):
     p = os.path.join(OUT, f)

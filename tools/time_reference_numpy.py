@@ -1,8 +1,7 @@
-"""Times the UNMODIFIED reference's own NumPy `env.step()` (imported from /root/reference, build container only) on the
-BASELINE configurations, one process per allowed core, and writes profiles/reference_numpy_step.json - the number the
-north star asks to be reported beside the GPU rate.  The reference is pure Python and may neither be copied into this
-repo nor reached from the GPU box, so bench.py quotes this committed measurement (with its core count and host) instead
-of re-measuring it there.
+"""Times the UNMODIFIED reference's own NumPy `env.step()` (imported from a reference checkout, oracle/ref_harness.py) on
+the BASELINE configurations, one process per allowed core, and prints the rates as JSON - the number the north star asks
+to be reported beside the GPU rate.  The reference is pure Python and is not part of this repository, so it is timed
+wherever a checkout exists, with the host's core count stated.
 
     python tools/time_reference_numpy.py [--steps 300]
 """
@@ -67,8 +66,7 @@ def main():
         out["configs"][key] = {"env_steps_per_s_per_core": per_core, "env_steps_per_s_all_cores": float(np.sum(rates)),
                                "agent_env_steps_per_s_all_cores": float(np.sum(rates)) * agents[cfg], "n_agents": agents[cfg]}
         print(key, out["configs"][key], flush=True)
-    with open(os.path.join(ROOT, "profiles", "reference_numpy_step.json"), "w") as fh:
-        json.dump(out, fh, indent=1)
+    print(json.dumps(out, indent=1))
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
-// wpattern.cu — micro-benchmark: how fast can one warp per env stream its observation planes to HBM on B200,
+// wpattern.cu — micro-benchmark: how fast can one warp per env stream its observation planes to HBM on H100,
 // depending on the store pattern?  (Experiment behind DESIGN.md "observation write-out".)
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gpurun_out/wpattern tools/wpattern.cu && gpurun_out/wpattern
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/wpattern tools/wpattern.cu && /tmp/wpattern
 //
 // Every pattern writes the same bytes: per env a "planner map" of 6 planes x 625 floats followed by 4 "agent
 // windows" of 7 planes x 121 floats (28552 B), 8192 envs, 8 warps per CTA, 4 CTAs per SM (shared-memory limited,
