@@ -27,7 +27,8 @@ namespace be {
 constexpr int AIE_MAX_SLICES_BE = 16;   // = AIE_MAX_SLICES (aie_compact_host.h)
 struct State {
     int step_wpb;        // warps (envs) per CTA of the step kernel
-    int step_minb;       // register-allocation variant of the step kernel (3, 4 or 5 CTAs per SM)
+    int step_minb;       // register-allocation variant of the step kernel (3 or 4 CTAs per SM)
+    int step_cs;         // component set the step kernel is instantiated for (step_comp_set)
     size_t step_smem;    // dynamic shared memory per CTA
     int obs_threads;
     size_t obs_smem;
@@ -161,16 +162,64 @@ struct DevExec {
     int tid;
     __device__ __forceinline__ int nt() const { return NT; }
     __device__ __forceinline__ void sync() const { if (NT == 32) __syncwarp(); else __syncthreads(); }
-    template <class F> __device__ __forceinline__ void operator()(F f) const { f(tid); sync(); }
+    // one warp per env: the phase gets the lane re-read from %laneid, so no lane index stays live across phases
+    template <class F> __device__ __forceinline__ void operator()(F f) const { f(NT == 32 ? relane(tid) : tid); sync(); }
     // the record image's tail (price history, order slots) is about to be reused as staging memory
     __device__ __forceinline__ void record_stored() const {
         if (FUSED) { if (tid == 0) bulk_wait_read(); sync(); }
     }
 };
 
+// Auto-reset (WarpDrive save_copy_and_apply_at_reset semantics): restore everything but the RNG stream from the
+// load-time snapshot; the episode counters and the numpy stream carry on.  Once per episode: kept out of line so that
+// the step's hot text does not carry it.
+template <bool EXT>
+__device__ __noinline__ void auto_reset_env(const DevCfg &c, const DevBufs &b, int env, uint8_t *rec, uint64_t *bar, int lane) {
+    uint8_t *scratch = rec + c.resident_bytes;
+    uint8_t *grec = b.state + (size_t)env * c.rec_bytes;
+    int32_t *hdr = (int32_t *)rec;
+    const int32_t completions = hdr[HDR_COMPLETIONS] + 1, warm = hdr[HDR_AUTO_WARMUP], mt_pos = hdr[HDR_MT_POS],
+                  episodes = hdr[HDR_EPISODES] + 1, saez_n = hdr[HDR_SAEZ_N];
+    const uint8_t *snap = b.state0 + (size_t)env * c.rec_bytes;
+    const uint32_t tail = (uint32_t)(c.rec_bytes - c.off_price_hist);  // price history + order slots
+    fence_async_smem();
+    __syncwarp();
+    if (b.final && lane == 0) {  // end-of-episode snapshot (previous_episode_metrics): the resident record as it stands
+        bulk_s2g(b.final + (size_t)env * c.rec_bytes, rec, (uint32_t)c.resident_bytes);
+        bulk_wait_read();
+    }
+    if (b.final && c.split) {  // the statistics of a split record live in global memory
+        const uint4 *src = (const uint4 *)(grec + c.off_stats);
+        uint4 *dst = (uint4 *)(b.final + (size_t)env * c.rec_bytes + c.off_stats);
+        for (int i = lane; i < (8 * c.n_stats + 15) / 16; i += 32) dst[i] = src[i];
+    }
+    __syncwarp();
+    if (lane == 0) {
+        mbar_expect_tx(bar, (uint32_t)c.off_mt + (c.split ? 0u : tail));
+        bulk_g2s(rec, snap, (uint32_t)c.off_mt, bar);
+        if (!c.split) bulk_g2s(rec + c.off_price_hist, snap + c.off_price_hist, tail, bar);
+    }
+    if (c.split) {  // the big sections live in global memory: copy them back from the snapshot with plain stores
+        const uint4 *src = (const uint4 *)(snap + c.off_price_hist);
+        uint4 *dst = (uint4 *)(grec + c.off_price_hist);
+        for (uint32_t i = lane; i < tail / 16; i += 32) dst[i] = src[i];
+    }
+    __syncwarp();
+    mbar_wait(bar, 1);
+    if (lane == 0) {
+        hdr[HDR_COMPLETIONS] = completions; hdr[HDR_AUTO_WARMUP] = warm; hdr[HDR_MT_POS] = mt_pos;
+        hdr[HDR_EPISODES] = episodes; hdr[HDR_SAEZ_N] = saez_n;
+    }
+    __syncwarp();
+    if (c.reset_mode == 1)   // reference-exact layout (dynamic scenarios) / placement / skills
+        device_reset_env<EXT>(c, rec, grec, scratch, lane, b.dyn_prob, b.dyn_work ? b.dyn_work + (size_t)env * (c.HW + 16) : nullptr);
+    finish_reset_env(c, rec, grec, scratch, lane);  // metric_0 under the new completions count
+}
+
 // One warp: bulk-load env's record, advance it one timestep (auto-reset included), start the write-back.  On return the
 // record image is final; with obs_alias_mt the MT19937 key went out as its own first group and has been read already.
-template <bool BIG, bool EXT>
+// CS: the component kinds compiled into the step body (step_comp_set).
+template <bool BIG, bool EXT, int CS = CS_ALL>
 __device__ __forceinline__ void warp_step(const DevCfg &c, const DevBufs &b, int env, uint8_t *rec, uint64_t *bar,
                                           const uint16_t *tab, int lane) {
     uint8_t *scratch = rec + c.resident_bytes;
@@ -188,50 +237,10 @@ __device__ __forceinline__ void warp_step(const DevCfg &c, const DevBufs &b, int
     mbar_wait(bar, 0);
 
     int32_t *events = (b.events && env < b.event_envs) ? b.events + (size_t)env * 8 * (b.event_cap + 1) : nullptr;
-    step_env<BIG, EXT>(c, rec, grec, scratch, act_a, act_p, b.rew + (size_t)env * (c.A + 1), b.done + env, lane, true, events,
-                  b.event_cap);
-
-    // auto-reset (WarpDrive save_copy_and_apply_at_reset semantics): restore everything but the RNG stream
-    // from the load-time snapshot; the episode counters and the numpy stream carry on.
-    int32_t *hdr = (int32_t *)rec;
-    if (c.auto_reset && hdr[HDR_T] >= c.T) {
-        const int32_t completions = hdr[HDR_COMPLETIONS] + 1, warm = hdr[HDR_AUTO_WARMUP], mt_pos = hdr[HDR_MT_POS],
-                      episodes = hdr[HDR_EPISODES] + 1, saez_n = hdr[HDR_SAEZ_N];
-        const uint8_t *snap = b.state0 + (size_t)env * c.rec_bytes;
-        const uint32_t tail = (uint32_t)(c.rec_bytes - c.off_price_hist);  // price history + order slots
-        fence_async_smem();
-        __syncwarp();
-        if (b.final && lane == 0) {  // end-of-episode snapshot (previous_episode_metrics): the resident record as it stands
-            bulk_s2g(b.final + (size_t)env * c.rec_bytes, rec, (uint32_t)c.resident_bytes);
-            bulk_wait_read();
-        }
-        if (b.final && c.split) {  // the statistics of a split record live in global memory
-            const uint4 *src = (const uint4 *)(grec + c.off_stats);
-            uint4 *dst = (uint4 *)(b.final + (size_t)env * c.rec_bytes + c.off_stats);
-            for (int i = lane; i < (8 * c.n_stats + 15) / 16; i += 32) dst[i] = src[i];
-        }
-        __syncwarp();
-        if (lane == 0) {
-            mbar_expect_tx(bar, (uint32_t)c.off_mt + (c.split ? 0u : tail));
-            bulk_g2s(rec, snap, (uint32_t)c.off_mt, bar);
-            if (!c.split) bulk_g2s(rec + c.off_price_hist, snap + c.off_price_hist, tail, bar);
-        }
-        if (c.split) {  // the big sections live in global memory: copy them back from the snapshot with plain stores
-            const uint4 *src = (const uint4 *)(snap + c.off_price_hist);
-            uint4 *dst = (uint4 *)(grec + c.off_price_hist);
-            for (uint32_t i = lane; i < tail / 16; i += 32) dst[i] = src[i];
-        }
-        __syncwarp();
-        mbar_wait(bar, 1);
-        if (lane == 0) {
-            hdr[HDR_COMPLETIONS] = completions; hdr[HDR_AUTO_WARMUP] = warm; hdr[HDR_MT_POS] = mt_pos;
-            hdr[HDR_EPISODES] = episodes; hdr[HDR_SAEZ_N] = saez_n;
-        }
-        __syncwarp();
-        if (c.reset_mode == 1)   // reference-exact layout (dynamic scenarios) / placement / skills
-            device_reset_env<EXT>(c, rec, grec, scratch, lane, b.dyn_prob, b.dyn_work ? b.dyn_work + (size_t)env * (c.HW + 16) : nullptr);
-        finish_reset_env(c, rec, grec, scratch, lane);  // metric_0 under the new completions count
-    }
+    step_env<BIG, EXT, CS>(c, rec, grec, scratch, act_a, act_p, b.rew + (size_t)env * (c.A + 1), b.done + env, lane, true,
+                           events, b.event_cap);
+    lane = relane(lane);
+    if (c.auto_reset && ((const int32_t *)rec)[HDR_T] >= c.T) auto_reset_env<EXT>(c, b, env, rec, bar, lane);
 
     fence_async_smem();  // generic-proxy writes to the record -> visible to the bulk (async-proxy) store
     __syncwarp();
@@ -256,8 +265,8 @@ __device__ __forceinline__ void warp_step(const DevCfg &c, const DevBufs &b, int
 
 // ---------------------------------------------------------------------------------------------------------
 // One warp per env, up to 8 envs per CTA.  MINB = minimum resident CTAs per SM the register allocation targets
-// (occupancy vs. registers per thread).
-template <int MINB, bool EXT = false>
+// (occupancy vs. registers per thread); CS = the component kinds compiled in (step_comp_set).
+template <int MINB, bool EXT, int CS>
 __global__ void __launch_bounds__(256, MINB) aie_step_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
                                                               const int emit_obs, const int env_lo) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -268,9 +277,9 @@ __global__ void __launch_bounds__(256, MINB) aie_step_kernel(const __grid_consta
     if (env >= c.n_envs && !phase_sync) return;  // from here on warps are independent: no block-wide barrier below
     uint64_t *bar = (uint64_t *)smem + warp;
     uint8_t *rec = warp_region(smem, wpb, warp, c);
-    if (env < c.n_envs) warp_step<false, EXT>(c, b, env, rec, bar, tab, lane);
+    if (env < c.n_envs) warp_step<false, EXT, CS>(c, b, env, rec, bar, tab, lane);
     if (phase_sync) { __syncthreads(); if (env >= c.n_envs) return; }
-    if (emit_obs & 1) observe_env<EXT>(c, rec, b.state + (size_t)env * c.rec_bytes, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<32, true>{lane});
+    if (emit_obs & 1) observe_env<EXT, CS>(c, rec, b.state + (size_t)env * c.rec_bytes, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<32, true>{lane});
     else if (lane == 0) bulk_wait_read();
 }
 
@@ -425,14 +434,17 @@ int init(aie_env *env) {
     env->be.obs_threads = wpb * 32;
     env->be.obs_smem = env->be.step_smem;
     // Register budget: the 64-register variant (launch bounds 256 x 4) when more than 24 warps can be resident (c2: 32
-    // warps per SM), otherwise the 80-register variant, which does not spill.  Override: AIE_STEP_MINB=3|4|5.  This rule
-    // and the envs-per-CTA search above are carried over from the kernels' first target (same 228 KB of shared memory and
-    // 64 K registers per SM as the H100); they have not been re-tuned on the H100.
+    // warps per SM), otherwise the 80-register variant (c3: 20 warps).  Override: AIE_STEP_MINB=3|4.  Measured on an
+    // H100 80GB HBM3 (700 W), one 300-step run per setting, step kernel: c2 248 us with 64 registers vs 305 us with 80;
+    // c3 511 us with 80 vs 539 us with 64.  Envs per CTA stay at the search above: c2 at 4 per CTA took 248 us, as at
+    // 8.  c3 at 2 per CTA, alternated five times with 8 on an H100 80GB HBM3 (400 W), took 0.4870 ms / step (range
+    // 0.4854-0.4871) vs 0.4879 (0.4863-0.4883), while its step kernel timed alone took 532 us vs 502 us: no clear gain.
     const size_t smem_sm = prop.sharedMemPerMultiprocessor;
     int fit = (int)(smem_sm / (env->be.step_smem + 1024));
     const int resident_warps = (fit * wpb > 32) ? 32 : fit * wpb;
     env->be.step_minb = resident_warps > 24 ? 4 : 3;
-    if (const char *ov = getenv("AIE_STEP_MINB")) { int v = atoi(ov); if (v >= 3 && v <= 5) env->be.step_minb = v; }
+    if (const char *ov = getenv("AIE_STEP_MINB")) { int v = atoi(ov); if (v == 3 || v == 4) env->be.step_minb = v; }
+    env->be.step_cs = step_comp_set(c);
     if (getenv("AIE_VERBOSE"))
         fprintf(stderr, "[aie] record %d B (resident %d, obs prefix %d), step scratch %d, obs scratch %d (alias mt %d), per env %zu B, "
                         "%d envs/CTA, %zu B smem/CTA, register variant %d, %d CTAs/SM fit\n", c.rec_bytes, c.resident_bytes, c.obs_prefix_bytes,
@@ -441,8 +453,10 @@ int init(aie_env *env) {
     // record must not lower it under the first one, so every kernel is simply opted in to the device maximum.
     const int sm = (int)max_smem;
 #define AIE_OPT_IN(k) AIE_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, sm), "smem attr")
-    AIE_OPT_IN((aie_step_kernel<3, false>)); AIE_OPT_IN((aie_step_kernel<4, false>)); AIE_OPT_IN((aie_step_kernel<5, false>));
-    AIE_OPT_IN((aie_step_kernel<3, true>)); AIE_OPT_IN((aie_step_kernel<4, true>));
+    AIE_OPT_IN((aie_step_kernel<3, false, CS_GTB>)); AIE_OPT_IN((aie_step_kernel<4, false, CS_GTB>));
+    AIE_OPT_IN((aie_step_kernel<3, false, CS_GTB_TAX>)); AIE_OPT_IN((aie_step_kernel<4, false, CS_GTB_TAX>));
+    AIE_OPT_IN((aie_step_kernel<3, false, CS_ALL>)); AIE_OPT_IN((aie_step_kernel<4, false, CS_ALL>));
+    AIE_OPT_IN((aie_step_kernel<3, true, CS_ALL>)); AIE_OPT_IN((aie_step_kernel<4, true, CS_ALL>));
     AIE_OPT_IN((aie_step_mw_kernel<false, false>)); AIE_OPT_IN((aie_step_mw_kernel<false, true>));
     AIE_OPT_IN((aie_step_mw_kernel<true, false>)); AIE_OPT_IN((aie_step_mw_kernel<true, true>));
     AIE_OPT_IN(aie_finish_reset_kernel);
@@ -603,12 +617,15 @@ int launch_step_range(aie_env *env, int emit_obs, int lo, int hi, void *stream) 
         else aie_step_mw_kernel<false, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
     } else {
         const dim3 grid((n + wpb - 1) / wpb), block(wpb * 32);
-        if (env->cfg.ext) {  // rarely used options compiled in (single-action planner, regen halfwidth); 48-register variant omitted
-            if (env->be.step_minb >= 4) aie_step_kernel<4, true><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
-            else aie_step_kernel<3, true><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
-        } else if (env->be.step_minb == 5) aie_step_kernel<5, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
-        else if (env->be.step_minb == 4) aie_step_kernel<4, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
-        else aie_step_kernel<3, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
+        const bool m4 = env->be.step_minb == 4;
+#define AIE_STEP(EXT, CS) (m4 ? aie_step_kernel<4, EXT, CS><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo) \
+                              : aie_step_kernel<3, EXT, CS><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo))
+        // EXT: rarely used options compiled in (single-action planner, regen halfwidth), with every component kind
+        if (env->cfg.ext) AIE_STEP(true, CS_ALL);
+        else if (env->be.step_cs == CS_GTB) AIE_STEP(false, CS_GTB);
+        else if (env->be.step_cs == CS_GTB_TAX) AIE_STEP(false, CS_GTB_TAX);
+        else AIE_STEP(false, CS_ALL);
+#undef AIE_STEP
     }
     AIE_CUDA(cudaGetLastError(), "aie_step_kernel launch");
     env->launches++;

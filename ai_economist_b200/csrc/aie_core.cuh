@@ -61,6 +61,10 @@ AIE_DEV double wsum(double v) {
     return v;
 }
 AIE_DEV int first_lane(uint32_t m) { return __ffs(m) - 1; }
+// The calling thread's lane, read afresh from %laneid (volatile: never merged with an earlier read).  A lane index kept
+// live through the whole step is the value the 64-register variant spills first; re-reading it at the start of each
+// component / observation phase keeps its live ranges short.  `lane` is the value the caller holds (host emulation).
+AIE_DEV int relane(int) { int l; asm volatile("mov.u32 %0, %%laneid;" : "=r"(l)); return l; }
 AIE_DEV int __popc_u32(uint32_t m) { return __popc(m); }
 AIE_DEV uint32_t fshr(uint32_t lo, uint32_t hi, int sh) { return __funnelshift_r(lo, hi, sh); }  // sh in [0, 31]
 AIE_DEV uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) { return __byte_perm(a, b, sel); }
@@ -76,6 +80,7 @@ AIE_DEV uint32_t wshfl(uint32_t v, int) { return v; }
 AIE_DEV bool wany(bool p) { return p; }
 AIE_DEV double wsum(double v) { return v; }
 AIE_DEV int first_lane(uint32_t m) { return m ? 0 : -1; }
+AIE_DEV int relane(int lane) { return lane; }
 AIE_DEV int __popc_u32(uint32_t m) { return __builtin_popcount(m); }
 AIE_DEV uint32_t fshr(uint32_t lo, uint32_t hi, int sh) { return sh ? (lo >> sh) | (hi << (32 - sh)) : lo; }
 AIE_DEV uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
@@ -137,14 +142,29 @@ AIE_DEV Env env_view(uint8_t *rec, uint8_t *grec, const DevCfg &c) {
     return e;
 }
 
+// Component sets the step body can be compiled for (bit k: component kind k is handled).  The one-warp step kernel is
+// instantiated per set and the host launches the smallest set that holds the config's components, so a config without
+// taxes does not carry the tax code inside its hot loops.
+constexpr int CS_GTB = (1 << COMP_BUILD) | (1 << COMP_CDA) | (1 << COMP_GATHER);   // gather-trade-build
+constexpr int CS_GTB_TAX = CS_GTB | (1 << COMP_TAX);
+constexpr int CS_ALL = (1 << COMP_KINDS) - 1;
+inline int step_comp_set(const DevCfg &c) {
+    int m = 0;
+    for (int i = 0; i < c.n_comp; i++) m |= 1 << c.comp[i];
+    return (m & ~CS_GTB) == 0 ? CS_GTB : (m & ~CS_GTB_TAX) == 0 ? CS_GTB_TAX : CS_ALL;
+}
+
 // Append one event row (called by the committing lane only).  Rows beyond the capacity are counted as dropped.
-AIE_DEV void emit_event(const Env &e, int kind, int a0, int a1 = 0, int a2 = 0, int a3 = 0, int a4 = 0, int a5 = 0, int a6 = 0) {
-    if (!e.ev) return;
-    const int n = e.ev[0];
-    if (n >= e.ev_cap) { e.ev[2] += 1; return; }
-    int32_t *row = e.ev + 8 * (n + 1);
+// Only the dense-log replicas have an event block: the row writer is kept out of line.
+AIE_DEV_NOINLINE void emit_event_row(int32_t *ev, int cap, int kind, int a0, int a1, int a2, int a3, int a4, int a5, int a6) {
+    const int n = ev[0];
+    if (n >= cap) { ev[2] += 1; return; }
+    int32_t *row = ev + 8 * (n + 1);
     row[0] = kind; row[1] = a0; row[2] = a1; row[3] = a2; row[4] = a3; row[5] = a4; row[6] = a5; row[7] = a6;
-    e.ev[0] = n + 1;
+    ev[0] = n + 1;
+}
+AIE_DEV void emit_event(const Env &e, int kind, int a0, int a1 = 0, int a2 = 0, int a3 = 0, int a4 = 0, int a5 = 0, int a6 = 0) {
+    if (e.ev) emit_event_row(e.ev, e.ev_cap, kind, a0, a1, a2, a3, a4, a5, a6);
 }
 
 // per-env scratch of the step body (shared memory on the device)
@@ -856,6 +876,38 @@ AIE_DEV double energy_weight(const DevCfg &c, const Env &e) {
     return 1.0 - exp(-n / c.warm_const);
 }
 
+// Gini coefficient of the endowments x_a = coin[a] + esc_coin[a], sort-based branch (A >= 30): rank each endowment,
+// scatter to sorted order (tmp[A]), then cumulative sums.  Warp-collective.  Inlined: large populations (c5) take it
+// every step.
+AIE_DEV double gini_sorted(const double *coin, const double *esc_coin, double *tmp, int A, int lane) {
+    for (int i = lane; i < A; i += NL) {
+        double xi = coin[i] + esc_coin[i];
+        int rank = 0;
+        for (int j = 0; j < A; j++) {
+            double xj = coin[j] + esc_coin[j];
+            rank += (xj < xi || (xj == xi && j < i)) ? 1 : 0;
+        }
+        tmp[rank] = xi;
+    }
+    wsync();
+    double tot = 0.0, cum = 0.0, acc = 0.0;
+    for (int i = 0; i < A; i++) tot += tmp[i];
+    for (int i = 0; i < A; i++) { cum += tmp[i]; acc += cum / (tot + 1e-10); }
+    return 1.0 - (2.0 / (A + 1)) * acc;
+}
+// inv_income_weighted_coin_endowments (swf 1) / inv_income_weighted_utility (swf 2): weights 1 / max(x_a, 1), normalised.
+// Out of line: the benchmarked configurations use the default welfare function (coin_eq_times_productivity).
+AIE_DEV_NOINLINE double inv_income_weighted(const double *coin, const double *esc_coin, const double *util, int A, int swf) {
+    double wsum_ = 0.0, acc = 0.0;
+    for (int a = 0; a < A; a++) wsum_ += 1.0 / fmax(coin[a] + esc_coin[a], 1.0);
+    for (int a = 0; a < A; a++) {
+        double x = coin[a] + esc_coin[a];
+        double wgt = (1.0 / fmax(x, 1.0)) / wsum_;
+        acc += (swf == 1 ? x : util[a]) * wgt;
+    }
+    return acc;
+}
+
 // Writes util[0..A] (agents, then planner) into `out` (scratch or record).  Warp-collective.
 AIE_DEV void current_metrics(const DevCfg &c, const Env &e, double *out, double *tmp, int lane) {
     const int A = c.A;
@@ -882,33 +934,13 @@ AIE_DEV void current_metrics(const DevCfg &c, const Env &e, double *out, double 
             }
             double diff = wsum(part);
             gini = (diff / (2 * A * total + 1e-10)) / ((A - 1) / (double)A);
-        } else {  // sort-based branch: rank each endowment, scatter to sorted order, then cumulative sums
-            for (int i = lane; i < A; i += NL) {
-                double xi = e.coin[i] + e.esc_coin[i];
-                int rank = 0;
-                for (int j = 0; j < A; j++) {
-                    double xj = e.coin[j] + e.esc_coin[j];
-                    rank += (xj < xi || (xj == xi && j < i)) ? 1 : 0;
-                }
-                tmp[rank] = xi;
-            }
-            wsync();
-            double tot = 0.0, cum = 0.0, acc = 0.0;
-            for (int i = 0; i < A; i++) tot += tmp[i];
-            for (int i = 0; i < A; i++) { cum += tmp[i]; acc += cum / (tot + 1e-10); }
-            gini = 1.0 - (2.0 / (A + 1)) * acc;
+        } else {
+            gini = gini_sorted(e.coin, e.esc_coin, tmp, A, lane);
         }
         double eqw = 1.0 - c.mix;
         planner = (eqw * (1.0 - gini) + (1.0 - eqw)) * (total / A);
     } else {
-        double wsum_ = 0.0, acc = 0.0;
-        for (int a = 0; a < A; a++) wsum_ += 1.0 / fmax(e.coin[a] + e.esc_coin[a], 1.0);
-        for (int a = 0; a < A; a++) {
-            double x = e.coin[a] + e.esc_coin[a];
-            double wgt = (1.0 / fmax(x, 1.0)) / wsum_;
-            acc += (c.swf == 1 ? x : out[a]) * wgt;
-        }
-        planner = acc;
+        planner = inv_income_weighted(e.coin, e.esc_coin, out, A, c.swf);
     }
     wsync();
     if (lane == 0) out[A] = planner;
@@ -1018,9 +1050,10 @@ AIE_DEV void compute_reward(const DevCfg &c, Env &e, const StepScratch &s, doubl
 }
 
 // ------------------------------------------------------------------------------------------------
-// One env.step() (base/base_env.py:929-1032) without the observation pass.
+// One env.step() (base/base_env.py:929-1032) without the observation pass.  CS: the component kinds compiled in
+// (a superset of the config's, see step_comp_set).
 // ------------------------------------------------------------------------------------------------
-template <bool BIG, bool EXT = false>
+template <bool BIG, bool EXT = false, int CS = CS_ALL>
 AIE_DEV void step_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *scratch, const int32_t *act_a,
                       const int32_t *act_p, double *rew_out, int32_t *done_out, int lane, bool decoded = false,
                       int32_t *events = nullptr, int event_cap = 0, const uint16_t *tab = nullptr) {
@@ -1036,21 +1069,28 @@ AIE_DEV void step_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *scr
     wsync();
     if (lane == 0) e.hdr[HDR_T] = t;
     for (int i = 0; i < c.n_comp; i++) {
+        lane = relane(lane); r.lane = lane;
         switch (c.comp[i]) {
-            case COMP_BUILD: build_step(c, e, s, r); break;
-            case COMP_CDA: cda_create<BIG>(c, e, s, t, lane); cda_match<BIG>(c, e, s, t, lane); cda_expire<BIG>(c, e, t, lane); break;
-            case COMP_GATHER: gather_step(c, e, s, r); break;
-            case COMP_TAX: tax_step<EXT>(c, e, s, r, lane); break;
-            case COMP_WEALTH: wealth_step(c, e, s, lane); break;
-            case COMP_LABOR: if (EXT) labor_step(c, e, s, r); break;
+            case COMP_BUILD: if (CS & (1 << COMP_BUILD)) build_step(c, e, s, r); break;
+            case COMP_CDA:
+                if (CS & (1 << COMP_CDA)) { cda_create<BIG>(c, e, s, t, lane); cda_match<BIG>(c, e, s, t, lane); cda_expire<BIG>(c, e, t, lane); }
+                break;
+            case COMP_GATHER: if (CS & (1 << COMP_GATHER)) gather_step(c, e, s, r); break;
+            case COMP_TAX: if (CS & (1 << COMP_TAX)) tax_step<EXT>(c, e, s, r, lane); break;
+            case COMP_WEALTH: if (CS & (1 << COMP_WEALTH)) wealth_step(c, e, s, lane); break;
+            case COMP_LABOR: if (EXT && (CS & (1 << COMP_LABOR))) labor_step(c, e, s, r); break;
         }
     }
 #if AIE_ON_DEVICE
 #pragma unroll 1
 #endif
-    for (int ri = 0; ri < 2; ri++)   // Wood, then Stone (one inlined copy); the one-step-economy has no map: scenario_step() is empty
+    for (int ri = 0; ri < 2; ri++) {  // Wood, then Stone (one inlined copy); the one-step-economy has no map: scenario_step() is empty
+        lane = relane(lane); r.lane = lane;
         if (!(EXT && c.one_step)) regen_resource<EXT>(c, e, 1 - ri, r);
+    }
+    lane = relane(lane);
     compute_reward<EXT>(c, e, s, rew_out, lane);
+    lane = relane(lane);
     if (lane == 0) {
         e.hdr[HDR_MT_POS] = r.pos;
         if (done_out) *done_out = (t >= c.T) ? 1 : 0;

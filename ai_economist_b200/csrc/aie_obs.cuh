@@ -369,7 +369,8 @@ AIE_DEV int policy_pick(const uint16_t *seg, int s0, int s1, const uint8_t *lim,
     return 0;
 }
 
-template <bool EXT, class Exec>
+// CS: the component kinds compiled in (see step_env)
+template <bool EXT, int CS = CS_ALL, class Exec>
 AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *stage_base, const int32_t *ob, const ObsOut &o,
                          const uint16_t *tab, const Exec &ex) {
     const Env e = env_view(rec, grec, c);
@@ -402,7 +403,7 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
                 s.shf[SH_PRICE_HIST + i] = (float)(acc * inv_scale);
             }
         }
-        if (c.has[COMP_TAX]) {  // redistribution.py:974-1023
+        if ((CS & (1 << COMP_TAX)) && c.has[COMP_TAX]) {  // redistribution.py:974-1023
             const int pos = e.hdr[HDR_TAX_POS];
             if (tid == 0) {
                 s.shf[SH_TAX_IS_TAX_DAY] = pos >= c.period ? 1.0f : 0.0f;
