@@ -29,6 +29,7 @@ struct State {
     int step_wpb;        // warps (envs) per CTA of the step kernel
     int step_minb;       // register-allocation variant of the step kernel (3 or 4 CTAs per SM)
     int step_cs;         // component set the step kernel is instantiated for (step_comp_set)
+    int phase_sync;      // 2 (AIE_PHASE_SYNC set): the warps of a CTA enter the fused observation pass together; else 0
     size_t step_smem;    // dynamic shared memory per CTA
     int obs_threads;
     size_t obs_smem;
@@ -326,13 +327,20 @@ __global__ void __launch_bounds__(256) aie_finish_reset_kernel(const __grid_cons
 }
 
 // Stand-alone observation pass (after a reset upload, or when the caller steps dynamics separately): bulk-loads only
-// the observable prefix of the record (+ the price history).  One warp per env, or (MW) one CTA of four warps per env.
+// what observe_env reads.  One warp per env, or (MW) one CTA of four warps per env.
+// observe_env reads the record's prefix [0, obs_prefix_bytes) and, outside it, only in phase A (before any staging
+// buffer that may overlap them is written):
+//   - the price history [off_price_hist, off_orders) (the auction's price_history / market_rate; in global memory when split);
+//   - the Saez section [off_saez, off_saez + 384) (tax_rate_observed: curr_rates, tax_marginal_rate: marginal_rate).
+// A field added to a phase-A read outside the prefix has to be added here (the emulation stages the same list).
 __device__ __forceinline__ void load_obs_prefix(const DevCfg &c, uint8_t *rec, const uint8_t *grec, uint64_t *bar) {
     const uint32_t ph = (uint32_t)(c.off_orders - c.off_price_hist);
+    const uint32_t saez = c.off_saez ? 8u * 48u : 0u;
     mbar_init(bar, 1);
-    mbar_expect_tx(bar, (uint32_t)c.obs_prefix_bytes + (c.split ? 0u : ph));
+    mbar_expect_tx(bar, (uint32_t)c.obs_prefix_bytes + (c.split ? 0u : ph) + saez);
     bulk_g2s(rec, grec, (uint32_t)c.obs_prefix_bytes, bar);
     if (!c.split) bulk_g2s(rec + c.off_price_hist, grec + c.off_price_hist, ph, bar);
+    if (saez) bulk_g2s(rec + c.off_saez, grec + c.off_saez, saez, bar);
 }
 template <bool EXT>
 __global__ void __launch_bounds__(256) aie_observe_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
@@ -445,10 +453,11 @@ int init(aie_env *env) {
     env->be.step_minb = resident_warps > 24 ? 4 : 3;
     if (const char *ov = getenv("AIE_STEP_MINB")) { int v = atoi(ov); if (v == 3 || v == 4) env->be.step_minb = v; }
     env->be.step_cs = step_comp_set(c);
+    env->be.phase_sync = getenv("AIE_PHASE_SYNC") ? 2 : 0;   // tuning aid, one-warp kernel only
     if (getenv("AIE_VERBOSE"))
-        fprintf(stderr, "[aie] record %d B (resident %d, obs prefix %d), step scratch %d, obs scratch %d (alias mt %d), per env %zu B, "
+        fprintf(stderr, "[aie] record %d B (resident %d, obs prefix %d), step scratch %d (alias mt %d), per env %zu B, "
                         "%d envs/CTA, %zu B smem/CTA, register variant %d, %d CTAs/SM fit\n", c.rec_bytes, c.resident_bytes, c.obs_prefix_bytes,
-                c.step_scratch_bytes, c.obs_scratch_bytes, c.obs_alias_mt, per_env, wpb, env->be.step_smem, env->be.step_minb, fit);
+                c.step_scratch_bytes, c.obs_alias_mt, per_env, wpb, env->be.step_smem, env->be.step_minb, fit);
     // The attribute belongs to the function (per device, process-wide), not to this handle: a second env with a smaller
     // record must not lower it under the first one, so every kernel is simply opted in to the device maximum.
     const int sm = (int)max_smem;
@@ -602,8 +611,7 @@ int launch_step_range(aie_env *env, int emit_obs, int lo, int hi, void *stream) 
     cudaStream_t st = (cudaStream_t)stream;
     const size_t sm = env->be.step_smem;
     if (lo < 0 || hi > env->n_envs || n <= 0) return fail(AIE_EINVAL, "launch_step_range: env range");
-    static const int phase_sync = getenv("AIE_PHASE_SYNC") ? 2 : 0;
-    if (env->cfg.mw == 1) emit_obs = (emit_obs ? 1 : 0) | phase_sync;
+    if (env->cfg.mw == 1) emit_obs = (emit_obs ? 1 : 0) | env->be.phase_sync;
     DevCfg ranged;
     const DevCfg *cp = &env->cfg;
     if (hi != env->n_envs) { ranged = env->cfg; ranged.n_envs = hi; cp = &ranged; }

@@ -469,7 +469,7 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
                 if (place(c.ob_chunk, fc, false) <= chunk_extra) { c.fl_chunk = fc; break; }
             place(c.ob_chunk, c.fl_chunk, true);
         }
-        {   // emulation: everything in a separate scratch allocation, nothing aliases the (live) record
+        {   // staging apart from the record (ob_emu): everything in one separate allocation, nothing aliases
             chunk_needs(c.ob_chunk);
             vals_needs(c.fl_chunk, false);
             int off = 0;

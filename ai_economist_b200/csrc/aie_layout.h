@@ -117,8 +117,9 @@ struct DevCfg {
     // history / order slots (kernel waits for the whole write-back to have been read first).  What does not fit goes to
     // obs_extra_bytes of additional shared memory per env.  The value staging of the flat vectors (OB_VALS) shares its bytes
     // with the window / plane buffers (OB_WC, OB_WI, OB_PL, OB_BITS): the flat runs are finished before those are first used.  ob[]: byte offsets from the env's shared-memory region
-    // (device); ob_emu[]: offsets inside a separate scratch allocation of obs_scratch_bytes (host emulation, where the
-    // record is live global memory and nothing may alias it).
+    // (the suite's host emulation, tests/emu, stages on an image of that region too).  ob_emu[]: offsets inside a separate
+    // scratch allocation of obs_scratch_bytes, for a host emulation that keeps the staging apart from a live record; no
+    // kernel reads them.
     int32_t obs_alias_mt, obs_extra_bytes;
     int32_t ob[OB_COUNT], ob_emu[OB_COUNT];
     int32_t ob_chunk;       // agents whose windows are staged / streamed together
@@ -129,7 +130,7 @@ struct DevCfg {
     // mw: warps cooperating on one env in the step / observe kernels (1: one warp per env, several envs per CTA;
     // 4: one CTA per env for large records - warp 0 runs the dynamics, all four stream the observations)
     int32_t mw;
-    // step-kernel scratch (per env, shared memory) and observe-kernel scratch
+    // step-kernel scratch (per env, shared memory, behind the record image); separate observation scratch (ob_emu[])
     int32_t step_scratch_bytes, obs_scratch_bytes;
     int32_t n_envs;
     int32_t sh_curr_rates, sh_last_incomes, sh_full, sh_count;  // offsets / size of the shared float staging array

@@ -299,8 +299,8 @@ struct ObsScratch {
     uint32_t *bits;       // concatenated bit string of the run being streamed
     float *vals;          // staged runs of the flat vectors / masks (shares its bytes with wc / wi / pl / bits)
 };
-// base: the env's shared-memory region on the device (offsets c.ob[] may alias dead parts of the record image), or a
-// separate scratch allocation in emulation (c.ob_emu[])
+// base: the env's shared-memory region (offsets c.ob[] may alias dead parts of the record image; the suite's host
+// emulation passes its image of that region), or a separate scratch allocation (c.ob_emu[])
 AIE_DEV ObsScratch obs_scratch_view(uint8_t *base, const int32_t *ob) {
     ObsScratch s;
     s.net_hist = (double *)(base + ob[OB_NET_HIST]);

@@ -98,19 +98,22 @@ def test_cuda_previous_episode_metrics_match_reference(path):
     _replay_previous_episode_metrics(path, None)
 
 
-@pytest.mark.parametrize("which", ["saez_reset", "saez_annealed_reset", "c3_reset", "c1_reset", "lognormal_reset", "us_federal_annealed"])
-def test_emulated_explicit_host_resets_match_reference(which):
+EXPLICIT = ["saez_reset", "saez_annealed_reset", "c3_reset", "c1_reset", "lognormal_reset", "us_federal_annealed"]
+
+
+def _replay_explicit_host_resets(which, factory):
     """auto_reset off: env.reset() between episodes goes through the host reset path.  It has to carry the Saez
     estimator's persistent state (sample counter, rates in force / observed) across the repacked records, and the
     completed-episode count that drives the tax-annealing and energy-warm-up schedules (c3_reset; base_env.py:1021-1025
-    increments it on the step that ends the episode)."""
-    from tests.emu.emu_stepper import emu_factory
+    increments it on the step that ends the episode).  Every reset ends in the stand-alone observation pass, which has to
+    stage the Saez section the curr_rates / marginal_rate observations read."""
     path = [p for p in FILES if which in p][0]
     z, meta, init = gu.load_fixture(path)
     kw = dict(meta["reference_kwargs"])
     name = kw.pop("scenario_name")
     kw["components"] = [tuple(c) for c in kw["components"]]
-    env = foundation.make_env_instance(name, n_envs=1, auto_reset=False, stepper_factory=emu_factory, **kw)
+    extra = dict(stepper_factory=factory) if factory else dict(device="cuda:0")
+    env = foundation.make_env_instance(name, n_envs=1, auto_reset=False, **kw, **extra)
     env.seed([meta["seed"]])
     env.reset()
     s = env.stepper
@@ -127,3 +130,15 @@ def test_emulated_explicit_host_resets_match_reference(which):
         st, ob = s.read_state(0), s.read_obs(0)
         ob["rew"], ob["done"] = last["rew"], last["done"]   # reward / done belong to the step, not to the reset
         gu.check_step(z, t, ob, st, full.get(t), "host-reset-trace", books=st["books"])
+
+
+@pytest.mark.parametrize("which", EXPLICIT)
+def test_emulated_explicit_host_resets_match_reference(which):
+    from tests.emu.emu_stepper import emu_factory
+    _replay_explicit_host_resets(which, emu_factory)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("which", EXPLICIT)
+def test_cuda_explicit_host_resets_match_reference(which):
+    _replay_explicit_host_resets(which, None)
