@@ -370,8 +370,8 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
         }
         // ---- observation staging (aie_obs.cuh: ObsScratch) ----
         const int ww = c.win * c.win, HW4 = (c.HW + 3) & ~3;
-        c.wc_stride = (ww + 7) & ~7;
-        c.wcu_magic = (c.wc_stride >> 3) > 1 ? (uint32_t)((1ull << 32) / (uint64_t)(c.wc_stride >> 3)) + 1u : 0u;
+        const int units = (ww + 7) >> 3;
+        c.wcu_magic = units > 1 ? (uint32_t)((1ull << 32) / (uint64_t)units) + 1u : 0u;
         c.pl_stride_a = 4 * ((ww + 31) / 32);
         c.pl_stride_p = 4 * ((c.HW + 31) / 32);
         int need[OB_COUNT];
@@ -383,36 +383,22 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
         need[OB_LOCMAP] = align16(HW4 + 8);
         const bool whole_map = c.planner_spatial || c.full_obs;
         auto chunk_needs = [&](int ac) {
-            need[OB_WC] = align16(ac * c.wc_stride + 16);
             need[OB_WI] = align16(std::max(ac * 2 * ww, c.full_obs ? 2 * HW4 : 0) + 16);
             need[OB_PL] = align16(std::max(ac * (c.M + 1) * c.pl_stride_a, whole_map ? c.M * c.pl_stride_p : 0) + 16);
             need[OB_BITS] = align16(4 * ((std::max(ac * (c.M + 1) * ww, whole_map ? c.M * c.HW : 0) + 31) / 32) + 16);
         };
         const int early_ids[] = {OB_NET_HIST, OB_SHF, OB_SC_A, OB_LIM, OB_PSH, OB_LOCMAP};
-        const int late_ids[] = {OB_WI, OB_PL, OB_BITS, OB_WC};
-        // a staged run of n floats may start up to 3 floats into its (16-byte aligned) staging area and is copied in
-        // whole 16-byte groups
-        auto pad_run = [](int n) { return (n + 6) & ~3; };
-        auto vals_needs = [&](int fc, bool commit) {
-            int off = 0, o[4];
-            o[0] = off; off += pad_run(fc * c.Fa);
-            o[1] = off; off += pad_run(fc * c.Na);
-            o[2] = off; off += pad_run(fc * c.Fpa);
-            o[3] = off; off += pad_run(c.Fp);
-            if (commit) for (int i = 0; i < 4; i++) c.vals_off[i] = o[i];
-            need[OB_VALS] = align16(4 * off + 16);
-        };
+        const int late_ids[] = {OB_WI, OB_PL, OB_BITS};
         // Device placement.  One region of the env's shared memory becomes free during the pass: [off_mt, resident + step
         // scratch).  Its first part, the MT19937 key image, is free from the start (the key goes out as its own bulk group);
         // the rest - the other kept state, price history, order slots, step scratch - once the scalars are staged and the
         // record's write-back has been read (DevExec::record_stored).  Early buffers (used before that point) therefore sit in
         // the key image, or in extra memory when they do not fit; the late buffers follow them and run on into extra memory
-        // behind the region as far as needed.  The flat-value staging shares its bytes with the window buffers.
+        // behind the region as far as needed.
         const int mt_lo = c.off_mt, mt_hi = c.off_mt + 4 * 624;
         const int scr_lo = c.resident_bytes, scr_hi = c.resident_bytes + c.step_scratch_bytes;
-        auto place = [&](int ac, int fc, bool commit) {
+        auto place = [&](int ac, bool commit) {
             chunk_needs(ac);
-            vals_needs(fc, commit);
             int off[OB_COUNT];
             // early buffers: first fit, largest first, into the key image and then into the step scratch (dead as soon as the
             // dynamics are done and never part of the write-back); if one does not fit, all of them go to extra memory
@@ -432,8 +418,7 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
             const int late_hi = (early_fits && cur_scr > scr_lo) ? scr_lo : scr_hi;
             int cur = late_lo;
             for (int id : late_ids) { off[id] = cur; cur += need[id]; }
-            off[OB_VALS] = late_lo;
-            int end = std::max(cur, late_lo + need[OB_VALS]);
+            int end = cur;
             int extra = 0;
             if (end > late_hi) {   // the overflow continues behind the whole region: shift what lies beyond late_hi
                 const int shift = scr_hi - late_hi;   // 0, or the scratch bytes the early buffers occupy
@@ -442,8 +427,7 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
                     // the whole late block behind the region
                     int c2 = scr_hi;
                     for (int id : late_ids) { off[id] = c2; c2 += need[id]; }
-                    off[OB_VALS] = scr_hi;
-                    end = std::max(c2, scr_hi + need[OB_VALS]);
+                    end = c2;
                 }
                 extra = end - scr_hi;
             }
@@ -456,22 +440,16 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
             return extra;
         };
         {
-            // agents per window chunk: the largest count (<= 16) whose staging needs no more shared memory than one agent's;
-            // agents per flat chunk: likewise, given the window chunk
-            const int base_extra = place(1, 1, false);
+            // agents per window chunk: the largest count (<= 16) whose staging needs no more shared memory than one agent's
+            const int base_extra = place(1, false);
             int best = 0;
             for (int ac = std::min(A, 16); ac >= 1; ac--)
-                if (place(ac, 1, false) <= base_extra) { best = ac; break; }
+                if (place(ac, false) <= base_extra) { best = ac; break; }
             c.ob_chunk = best ? best : std::min(A, 4);
-            const int chunk_extra = place(c.ob_chunk, 1, false);
-            c.fl_chunk = 1;
-            for (int fc = A; fc >= 1; fc--)
-                if (place(c.ob_chunk, fc, false) <= chunk_extra) { c.fl_chunk = fc; break; }
-            place(c.ob_chunk, c.fl_chunk, true);
+            place(c.ob_chunk, true);
         }
         {   // staging apart from the record (ob_emu): everything in one separate allocation, nothing aliases
             chunk_needs(c.ob_chunk);
-            vals_needs(c.fl_chunk, false);
             int off = 0;
             for (int i = 0; i < OB_COUNT; i++) { c.ob_emu[i] = off; off += need[i]; }
             c.obs_scratch_bytes = off;

@@ -59,7 +59,7 @@ enum { SUB_BUILD = 0, SUB_BUY = 1, SUB_SELL = 2, SUB_GATHER = 3, SUB_LABOR = 4 }
 // mask segment = count << 8 | slot: `count` consecutive mask entries of one slot with idx 0 .. count-1 (random policy)
 enum { FK_SHARED = 0, FK_AGENT = 1, FK_MY = 2, FK_AVAIL = 3 };
 // observation staging buffers (see ObsScratch in aie_obs.cuh); offsets DevCfg::ob[] / ob_emu[]
-enum { OB_NET_HIST = 0, OB_SHF, OB_SC_A, OB_LIM, OB_PSH, OB_LOCMAP, OB_WC, OB_WI, OB_PL, OB_BITS, OB_VALS, OB_COUNT };
+enum { OB_NET_HIST = 0, OB_SHF, OB_SC_A, OB_LIM, OB_PSH, OB_LOCMAP, OB_WI, OB_PL, OB_BITS, OB_COUNT };
 enum { AS_LOC_ROW = 0, AS_LOC_COL, AS_INV_COIN, AS_INV_STONE, AS_INV_WOOD, AS_BUILD_PAYMENT, AS_BUILD_SKILL, AS_BONUS,
        AS_TAX_MARG, AS_TAX_LAST_INCOME, AS_TAX_LAST_MARG, AS_LABOR_SKILL /* one-step-economy */, AS_COUNT = 12 };
 enum { SH_ZERO = 0, SH_TIME = 1, SH_MARKET_RATE = 2, SH_ONE_PROD = 2, SH_ONE_EQ = 3 /* one-step-economy (no auction): planner scalars */, SH_TAX_IS_TAX_DAY = 4, SH_TAX_IS_FIRST = 5, SH_TAX_PHASE = 6,
@@ -115,17 +115,13 @@ struct DevCfg {
     // of DEAD parts of the record's shared-memory image: the MT19937 key (dead from the start of the pass: obs_alias_mt
     // != 0 makes the kernel write the key back as its own first bulk group) and, once the scalars are staged, the price
     // history / order slots (kernel waits for the whole write-back to have been read first).  What does not fit goes to
-    // obs_extra_bytes of additional shared memory per env.  The value staging of the flat vectors (OB_VALS) shares its bytes
-    // with the window / plane buffers (OB_WC, OB_WI, OB_PL, OB_BITS): the flat runs are finished before those are first used.  ob[]: byte offsets from the env's shared-memory region
+    // obs_extra_bytes of additional shared memory per env.  ob[]: byte offsets from the env's shared-memory region
     // (the suite's host emulation, tests/emu, stages on an image of that region too).  ob_emu[]: offsets inside a separate
     // scratch allocation of obs_scratch_bytes, for a host emulation that keeps the staging apart from a live record; no
     // kernel reads them.
     int32_t obs_alias_mt, obs_extra_bytes;
     int32_t ob[OB_COUNT], ob_emu[OB_COUNT];
     int32_t ob_chunk;       // agents whose windows are staged / streamed together
-    int32_t fl_chunk;       // agents whose flat vectors / masks / p<i> rows are staged (OB_VALS) and copied out together
-    int32_t vals_off[4];    // float offsets inside OB_VALS of the four staged runs: agent flat rows, agent mask rows, p<i> rows, planner flat
-    int32_t wc_stride;      // bytes per agent of the window-cell staging (window cells rounded up to 8)
     int32_t pl_stride_a, pl_stride_p;   // bytes per plane-local bitmap: one agent window / the whole map
     // mw: warps cooperating on one env in the step / observe kernels (1: one warp per env, several envs per CTA;
     // 4: one CTA per env for large records - warp 0 runs the dynamics, all four stream the observations)
@@ -140,7 +136,7 @@ struct DevCfg {
     int32_t cf_n_sh, cf_n_ag, cf_n_cnt;                // entries per class of the agents' flat vector
     int32_t seg_lo[10];                                // mask segments of action subspace si: [seg_lo[si], seg_lo[si + 1]) (single-action agents: si = 0 covers everything)
     uint32_t HW_magic, ww_magic, Fa_magic, Fpa_magic, Na_magic;  // floor(2^32 / n) + 1: run index -> (row, column)
-    uint32_t wcu_magic;     // floor(2^32 / (wc_stride / 8)) + 1: (agent, 8-cell unit) pairs of a chunk
+    uint32_t wcu_magic;     // floor(2^32 / units) + 1, units = ceil(window cells / 8): (agent, 8-cell unit) pairs of a chunk
     uint32_t win_magic; int32_t win_dr32, win_dc32;  // window walk: lane / win, and the (row, col) step of 32 cells
     // single-action planner (multi_action_mode_planner=False): act_p is one index into [NO-OP] ++ B x R rates
     int32_t planner_single;

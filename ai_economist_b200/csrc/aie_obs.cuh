@@ -72,35 +72,40 @@ AIE_DEV void store_edges(T *dst, const RunSplit &r, int n, int tid, int NT, F va
     const int ne = r.head + (n - r.tail0);
     for (int j = tid; j < ne; j += NT) { const int i = j < r.head ? j : r.tail0 + (j - r.head); dst[i] = (T)value_at(i); }
 }
-template <typename F>
-AIE_DEV void store_run_f32(float *dst, int n, int tid, int NT, F value_at) {
-    const RunSplit r = run_split(dst, n, 2);
-    store_edges(dst, r, n, tid, NT, value_at);
-#if AIE_ON_DEVICE
-    AIE_UNROLL(1)
-#endif
-    for (int g = tid; g < r.nq; g += NT) {
-        const int i0 = r.head + 4 * g;
-        store4(dst + i0, value_at(i0), value_at(i0 + 1), value_at(i0 + 2), value_at(i0 + 3));
-    }
-}
-// rows x n matrix, contiguous: dst[row * n + i] = value_at(row, i), written as ONE run (n_magic = floor(2^32 / n) + 1)
+// rows x n matrix, contiguous: dst[row * n + i] = value_at(row, i), written as ONE run (n_magic = floor(2^32 / n) + 1; not
+// read when rows == 1).  Thread tid owns the 16-byte groups tid, tid + NT, ... of the destination: it computes the group's
+// values in registers, one after the other through a single value_at site (the small code matters more than the three
+// moves per value), and stores them as one float4, or one by one for the <= 2 groups at the ends of the run.
 template <typename F>
 AIE_DEV void store_rows_f32(float *dst, int rows, int n, uint32_t n_magic, int tid, int NT, F value_at) {
     const int total = rows * n;
-    auto flat_value = [&](int x) { const int row = (int)div_magic((uint32_t)x, n_magic); return value_at(row, x - row * n); };
-    if (n < 4) { for (int x = tid; x < total; x += NT) dst[x] = flat_value(x); return; }
-    const RunSplit r = run_split(dst, total, 2);
-    store_edges(dst, r, total, tid, NT, flat_value);
+    const int a = (int)(((uintptr_t)dst >> 2) & 3);   // floats in front of the run inside its first 16-byte group
+    const int ng = (a + total + 3) >> 2;
 #if AIE_ON_DEVICE
     AIE_UNROLL(1)
 #endif
-    for (int g = tid; g < r.nq; g += NT) {
-        const int x0 = r.head + 4 * g;
-        const int row = (int)div_magic((uint32_t)x0, n_magic), i = x0 - row * n;
-        float v[4];
-        for (int j = 0; j < 4; j++) { const bool nx = i + j >= n; v[j] = value_at(nx ? row + 1 : row, nx ? i + j - n : i + j); }
-        store4(dst + x0, v[0], v[1], v[2], v[3]);
+    for (int k = tid; k < ng; k += NT) {
+        const int x0 = 4 * k - a;   // run index of the group's first float (negative in the first group when a > 0)
+        const int xs = x0 > 0 ? x0 : 0;
+        int row = rows > 1 ? (int)div_magic((uint32_t)xs, n_magic) : 0, i = xs - row * n;
+        float v0 = 0.0f, v1 = 0.0f, v2 = 0.0f, v3 = 0.0f;
+#if AIE_ON_DEVICE
+        AIE_UNROLL(1)
+#endif
+        for (int x = x0; x < x0 + 4; x++) {
+            float v = 0.0f;
+            if (x >= 0 && x < total) { v = value_at(row, i); if (++i == n) { i = 0; row++; } }
+            v0 = v1; v1 = v2; v2 = v3; v3 = v;
+        }
+        float *q = dst + x0;
+        if (x0 >= 0 && x0 + 4 <= total) {
+            store4(q, v0, v1, v2, v3);
+        } else {
+            if (x0 >= 0 && x0 < total) q[0] = v0;
+            if (x0 + 1 >= 0 && x0 + 1 < total) q[1] = v1;
+            if (x0 + 2 >= 0 && x0 + 2 < total) q[2] = v2;
+            if (x0 + 3 < total) q[3] = v3;
+        }
     }
 }
 // dst[i] = code(bytes[i]) widened to int16, code = identity (OWNER == false) or the house-owner encoding of an
@@ -129,33 +134,6 @@ AIE_DEV void store_bytes_i16(int16_t *dst, int n, const uint8_t *bytes, int tid,
     }
 }
 
-// ---- staged runs ---------------------------------------------------------------------------------------------------
-// Small float tensors (flat vectors, masks) are first written element by element into shared memory, laid out exactly like
-// the output run and shifted so that the 16-byte groups of the destination are 16-byte groups of the staging area
-// (element x of the run at vals[a + x], a = the destination's offset inside its 16-byte group, in floats); a second phase
-// copies the run out front to back, whole groups as float4 and the <= 3 elements at either end one by one.
-AIE_DEV int run_align(const float *dst) { return (int)(((uintptr_t)dst >> 2) & 3); }
-AIE_DEV void copy_run_f32(float *dst, int total, const float *vals, int tid, int NT) {
-    const int a = run_align(dst);
-    float *g0 = dst - a;
-    const int ng = (a + total + 3) >> 2;
-#if AIE_ON_DEVICE
-    AIE_UNROLL(1)
-#endif
-    for (int k = tid; k < ng; k += NT) {
-        const int lo = 4 * k - a;   // run index of the group's first float
-        if (lo >= 0 && lo + 4 <= total) {
-#if AIE_ON_DEVICE
-            *reinterpret_cast<float4 *>(g0 + 4 * k) = *reinterpret_cast<const float4 *>(vals + 4 * k);
-#else
-            for (int j = 0; j < 4; j++) g0[4 * k + j] = vals[4 * k + j];
-#endif
-        } else {
-            for (int j = 0; j < 4; j++) if (lo + j >= 0 && lo + j < total) g0[4 * k + j] = vals[4 * k + j];
-        }
-    }
-}
-
 // ---- bit planes ----------------------------------------------------------------------------------------------------
 // 8x8 bit-matrix transpose of 8 bytes held little-endian in (lo, hi): afterwards byte k holds bit k of the 8 input bytes
 // (bit j of output byte k = bit k of input byte j).
@@ -176,21 +154,6 @@ AIE_DEV void planes_from_cells(const uint8_t *cells, int n, uint8_t *planes, int
         uint32_t lo = c32[2 * u], hi = c32[2 * u + 1];
         transpose8(lo, hi);
         uint8_t *q = planes + u;
-        for (int m = 0; m < np; m++) { q[0] = (uint8_t)prmt(lo, hi, ((m < 4 ? s0 : s1) >> (8 * (m & 3))) & 7u); q += stride; }
-    }
-}
-// the same for `count` cell arrays `cell_stride` bytes apart (cell_stride = 8 * units: a multiple of 8), array k's planes at
-// planes + k * np * stride: ONE loop over all (array, unit) pairs, units_magic = floor(2^32 / units) + 1
-AIE_DEV void planes_from_cells_multi(const uint8_t *cells, int units, uint32_t units_magic, int count, uint8_t *planes, int stride,
-                                     int np, const uint8_t *psh, int tid, int NT) {
-    const uint32_t *c32 = reinterpret_cast<const uint32_t *>(cells);
-    const uint32_t s0 = reinterpret_cast<const uint32_t *>(psh)[0], s1 = reinterpret_cast<const uint32_t *>(psh)[1];
-    const int total = count * units, blk = np * stride;
-    for (int t = tid; t < total; t += NT) {
-        const int k = (int)div_magic((uint32_t)t, units_magic), u = t - k * units;
-        uint32_t lo = c32[2 * t], hi = c32[2 * t + 1];   // arrays are contiguous: unit t of the concatenation
-        transpose8(lo, hi);
-        uint8_t *q = planes + k * blk + u;
         for (int m = 0; m < np; m++) { q[0] = (uint8_t)prmt(lo, hi, ((m < 4 ? s0 : s1) >> (8 * (m & 3))) & 7u); q += stride; }
     }
 }
@@ -293,11 +256,9 @@ struct ObsScratch {
     uint8_t *lim;         // [A][MS_COUNT] mask limits: mask[j] = idx_j < lim[slot_j]
     uint8_t *psh;         // [8] map plane -> bit index of the cell byte (maps.state order); plane M = bit 6 ("inside the world")
     uint8_t *locmap;      // [HW]  0 none, a+2
-    uint8_t *wc;          // [chunk][wc_stride] window cells of a chunk of agents: cell bits | 0x40 inside
     uint8_t *wi;          // [chunk][2][ww] owner code, agent-location code (the int16 index planes as bytes)
     uint8_t *pl;          // plane-local bitmaps (agent chunk: [chunk][M+1] planes of ww bits; planner: [M] planes of HW bits)
     uint32_t *bits;       // concatenated bit string of the run being streamed
-    float *vals;          // staged runs of the flat vectors / masks (shares its bytes with wc / wi / pl / bits)
 };
 // base: the env's shared-memory region (offsets c.ob[] may alias dead parts of the record image; the suite's host
 // emulation passes its image of that region), or a separate scratch allocation (c.ob_emu[])
@@ -309,11 +270,9 @@ AIE_DEV ObsScratch obs_scratch_view(uint8_t *base, const int32_t *ob) {
     s.lim = base + ob[OB_LIM];
     s.psh = base + ob[OB_PSH];
     s.locmap = base + ob[OB_LOCMAP];
-    s.wc = base + ob[OB_WC];
     s.wi = base + ob[OB_WI];
     s.pl = base + ob[OB_PL];
     s.bits = (uint32_t *)(base + ob[OB_BITS]);
-    s.vals = (float *)(base + ob[OB_VALS]);
     return s;
 }
 
@@ -510,12 +469,33 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
     // live on top of them: the record's write-back must have finished reading shared memory first.
     ex.record_stored();
 
-    // ---- phase B: the planner's flat vector (staged; copied out with the first agent chunk below), planner mask, policy ----
+    // ---- phase B: the flat vectors and masks (base_env.py:562-612, base_agent.py:440-460), the policy ----------------
+    // Every flat / mask tensor is ONE run written straight from the staged scalars / limits: the four values of a 16-byte
+    // group are computed in registers and stored together (store_rows_f32).
     ex([&](int tid) {
-        {
+        const float *shf = s.shf;
+        const uint8_t *hist = e.bid_hist;
+        const int sh_full = c.sh_full;
+        {   // the planner's flat vector
             const uint16_t *tp = tab + c.tab_p;
-            float *v = s.vals + c.vals_off[3] + run_align(o.p_flat());
-            for (int j = tid; j < c.Fp; j += NT) v[j] = flat_value(s.shf, s.shf, e.bid_hist, hoff, 0, c.sh_full, tp[j]);
+            store_rows_f32(o.p_flat(), 1, c.Fp, 0u, tid, NT, [&](int, int j) { return flat_value(shf, shf, hist, hoff, 0, sh_full, tp[j]); });
+        }
+        // agents' flat vectors: sorted-key concatenation
+        store_rows_f32(o.a_flat(), A, c.Fa, c.Fa_magic, tid, NT, [&](int a, int j) {
+            return flat_value(shf, s.sc_a + a * AS_COUNT, hist, hoff, a * P, sh_full, tab[j]);
+        });
+        {   // action masks: entry (slot, idx) is open iff idx < limit[agent][slot]
+            const uint16_t *mt = tab + c.tab_m;
+            store_rows_f32(o.a_mask(), A, c.Na, c.Na_magic, tid, NT, [&](int a, int j) {
+                const uint32_t en = mt[j];
+                return ((en & 255u) < s.lim[a * MS_COUNT + (en >> 8)]) ? 1.0f : 0.0f;
+            });
+        }
+        if (!EXT || c.Fpa > 0) {   // the planner's per-agent vectors p<i>
+            const uint16_t *tpa = tab + c.tab_pa;
+            store_rows_f32(o.p_agents(), A, c.Fpa, c.Fpa_magic, tid, NT, [&](int a, int j) {
+                return flat_value(shf, s.sc_a + a * AS_COUNT, hist, hoff, a * P, sh_full, tpa[j]);
+            });
         }
         if (c.planner_acts) {  // redistribution.py:1025-1104, multi-action planner: per bracket [1] ++ rates
             const bool first_day = e.hdr[HDR_TAX_POS] == 1;
@@ -573,51 +553,6 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
         }
     });
 
-    // ---- flat vectors / masks of the agents (base_env.py:562-612, base_agent.py:440-460), fl_chunk agents at a time:
-    // phase 1 stages the chunk's rows of the three tensors as runs, phase 2 copies them out
-    for (int a0 = 0; a0 < A; a0 += c.fl_chunk) {
-        const int na = (A - a0 < c.fl_chunk) ? A - a0 : c.fl_chunk;
-        float *d_flat = o.a_flat() + (size_t)a0 * c.Fa, *d_mask = o.a_mask() + (size_t)a0 * c.Na, *d_pa = o.p_agents() + (size_t)a0 * c.Fpa;
-        ex([&](int tid) {
-            const float *shf = s.shf;
-            const uint8_t *hist = e.bid_hist;
-            const int sh_full = c.sh_full;
-            {   // agents' flat vectors: sorted-key concatenation
-                float *v = s.vals + c.vals_off[0] + run_align(d_flat);
-                const int n = c.Fa, total = na * n;
-                for (int x = tid; x < total; x += NT) {
-                    const int al = (int)div_magic((uint32_t)x, c.Fa_magic), j = x - al * n, a = a0 + al;
-                    v[x] = flat_value(shf, s.sc_a + a * AS_COUNT, hist, hoff, a * P, sh_full, tab[j]);
-                }
-            }
-            {   // action masks: entry (slot, idx) is open iff idx < limit[agent][slot]
-                float *v = s.vals + c.vals_off[1] + run_align(d_mask);
-                const uint16_t *mt = tab + c.tab_m;
-                const int n = c.Na, total = na * n;
-                for (int x = tid; x < total; x += NT) {
-                    const int al = (int)div_magic((uint32_t)x, c.Na_magic), j = x - al * n;
-                    const uint32_t en = mt[j];
-                    v[x] = ((en & 255u) < s.lim[(a0 + al) * MS_COUNT + (en >> 8)]) ? 1.0f : 0.0f;
-                }
-            }
-            if (!EXT || c.Fpa > 0) {   // the planner's per-agent vectors p<i>
-                float *v = s.vals + c.vals_off[2] + run_align(d_pa);
-                const uint16_t *tpa = tab + c.tab_pa;
-                const int n = c.Fpa, total = na * n;
-                for (int x = tid; x < total; x += NT) {
-                    const int al = (int)div_magic((uint32_t)x, c.Fpa_magic), j = x - al * n, a = a0 + al;
-                    v[x] = flat_value(shf, s.sc_a + a * AS_COUNT, hist, hoff, a * P, sh_full, tpa[j]);
-                }
-            }
-        });
-        ex([&](int tid) {
-            copy_run_f32(d_flat, na * c.Fa, s.vals + c.vals_off[0], tid, NT);
-            copy_run_f32(d_mask, na * c.Na, s.vals + c.vals_off[1], tid, NT);
-            if (!EXT || c.Fpa > 0) copy_run_f32(d_pa, na * c.Fpa, s.vals + c.vals_off[2], tid, NT);
-            if (a0 == 0) copy_run_f32(o.p_flat(), c.Fp, s.vals + c.vals_off[3], tid, NT);
-        });
-    }
-
     if (EXT && c.no_spatial) return;   // one-step-economy: nothing spatial
 
     // ---- phase C: the planner's spatial tensors: M bit planes of the whole map + the two index planes -----------------
@@ -663,40 +598,55 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
     }
 
     // ---- phase D: agent windows (layout_from_file.py:468-515), a chunk of agents at a time ----------------------------
-    // per chunk: the window cells of its agents are staged as bytes (cell bits | inside flag, owner code, location code),
-    // transposed into plane-local bitmaps, concatenated, and streamed as ONE run of chunk x (M+1) x ww floats; the index
-    // planes of the chunk stream as one run of chunk x 2 x ww int16.
-    const int psa = c.pl_stride_a, wcs = c.wc_stride, np1 = M + 1;
+    // per chunk: a thread takes 8 consecutive window cells of one agent (an 8-cell unit), builds their cell bytes (cell bits
+    // | inside flag) in registers and transposes them straight into the plane-local bitmaps, staging the owner / location
+    // codes as bytes; the bitmaps are then concatenated and streamed as ONE run of chunk x (M+1) x ww floats, the index
+    // planes of the chunk as one run of chunk x 2 x ww int16.
+    const int psa = c.pl_stride_a, units = (ww + 7) >> 3, np1 = M + 1;
     for (int a0 = 0; a0 < A; a0 += c.ob_chunk) {
         const int na = (A - a0 < c.ob_chunk) ? A - a0 : c.ob_chunk;
         float *am = o.a_map() + (size_t)a0 * np1 * ww;
         int head = 0;
         const int nwords = bits_words_for(am, na * np1 * ww, &head);
         ex([&](int tid) {
-            const int total = na * ww;
-            for (int t = tid; t < total; t += NT) {   // one (agent, window cell) pair per thread and iteration
-                const int al = (int)div_magic((uint32_t)t, c.ww_magic), q = t - al * ww, a = a0 + al;
-                const int dr = (int)div_magic((uint32_t)q, c.win_magic), dc = q - dr * win;
-                const int r2 = e.loc[2 * a] - w + dr, c2 = e.loc[2 * a + 1] - w + dc;
-                uint32_t cb = 0; int vo = 0, vl = 0;
-                if ((unsigned)r2 < (unsigned)H && (unsigned)c2 < (unsigned)W) {
-                    const int k = r2 * W + c2;
-                    cb = e.cell[k] | 0x40u;
-                    const int ow = e.owner[k];
-                    vo = ow < 0 ? 0 : (ow == a ? 1 : ow + 2);
-                    vl = s.locmap[k];
-                    if (vl == a + 2) vl = 1;
+            const uint32_t s0 = reinterpret_cast<const uint32_t *>(s.psh)[0], s1 = reinterpret_cast<const uint32_t *>(s.psh)[1];
+            const int total = na * units;
+            for (int t = tid; t < total; t += NT) {   // one (agent, 8-cell unit) pair per thread and iteration
+                const int al = (int)div_magic((uint32_t)t, c.wcu_magic), u = t - al * units, a = a0 + al, q0 = 8 * u;
+                int dr = (int)div_magic((uint32_t)q0, c.win_magic), dc = q0 - dr * win;
+                const int r0 = e.loc[2 * a] - w, c0 = e.loc[2 * a + 1] - w;
+                uint8_t *wi = s.wi + al * 2 * ww;
+                uint32_t lo = 0u, hi = 0u;   // the unit's cell bytes, shifted in from the top (cells past ww are 0)
+#if AIE_ON_DEVICE
+                AIE_UNROLL(1)
+#endif
+                for (int q = q0; q < q0 + 8; q++) {
+                    uint32_t cb = 0;
+                    if (q < ww) {
+                        const int r2 = r0 + dr, c2 = c0 + dc;
+                        int vo = 0, vl = 0;
+                        if ((unsigned)r2 < (unsigned)H && (unsigned)c2 < (unsigned)W) {
+                            const int k = r2 * W + c2;
+                            cb = e.cell[k] | 0x40u;
+                            const int ow = e.owner[k];
+                            vo = ow < 0 ? 0 : (ow == a ? 1 : ow + 2);
+                            vl = s.locmap[k];
+                            if (vl == a + 2) vl = 1;
+                        }
+                        wi[q] = (uint8_t)vo; wi[ww + q] = (uint8_t)vl;
+                        if (++dc == win) { dc = 0; dr++; }
+                    }
+                    lo = fshr(lo, hi, 8); hi = fshr(hi, cb, 8);
                 }
-                s.wc[al * wcs + q] = (uint8_t)cb;
-                uint8_t *wi = s.wi + al * 2 * ww + q;
-                wi[0] = (uint8_t)vo; wi[ww] = (uint8_t)vl;
+                transpose8(lo, hi);
+                uint8_t *pq = s.pl + al * np1 * psa + u;
+                for (int m = 0; m < np1; m++) { pq[0] = (uint8_t)prmt(lo, hi, ((m < 4 ? s0 : s1) >> (8 * (m & 3))) & 7u); pq += psa; }
             }
         });
         ex([&](int tid) {
-            planes_from_cells_multi(s.wc, wcs >> 3, c.wcu_magic, na, s.pl, psa, np1, s.psh, tid, NT);
             store_bytes_i16<false>(o.a_idx() + (size_t)a0 * 2 * ww, na * 2 * ww, s.wi, tid, NT);
+            concat_planes(s.bits, nwords, head, s.pl, psa, na * np1, ww, c.ww_magic, tid, NT);
         });
-        ex([&](int tid) { concat_planes(s.bits, nwords, head, s.pl, psa, na * np1, ww, c.ww_magic, tid, NT); });
         ex([&](int tid) { stream_bits_f32(am, na * np1 * ww, s.bits, lut, s.pl, psa, ww, c.ww_magic, tid, NT); });
     }
 }
