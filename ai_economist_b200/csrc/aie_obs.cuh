@@ -44,16 +44,19 @@ AIE_DEV RunSplit run_split(const void *dst, int n, int elem_log2) {
     r.tail0 = r.head + r.nq * per;
     return r;
 }
+// The 16-byte output stores are streaming stores (st.global.cs, evict-first): the outputs are written once per step and
+// are several times the size of L2, so kept at normal priority they would push the env records (read and written back
+// by the next step) out of L2.
 AIE_DEV void store4(float *p, float v0, float v1, float v2, float v3) {
 #if AIE_ON_DEVICE
-    *reinterpret_cast<float4 *>(p) = make_float4(v0, v1, v2, v3);
+    __stcs(reinterpret_cast<float4 *>(p), make_float4(v0, v1, v2, v3));
 #else
     p[0] = v0; p[1] = v1; p[2] = v2; p[3] = v3;
 #endif
 }
 AIE_DEV void store8(int16_t *p, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3) {  // 8 int16, little endian
 #if AIE_ON_DEVICE
-    *reinterpret_cast<uint4 *>(p) = make_uint4(w0, w1, w2, w3);
+    __stcs(reinterpret_cast<uint4 *>(p), make_uint4(w0, w1, w2, w3));
 #else
     const uint32_t w[4] = {w0, w1, w2, w3};
     for (int j = 0; j < 8; j++) p[j] = (int16_t)((w[j >> 1] >> (16 * (j & 1))) & 0xFFFFu);
@@ -227,12 +230,12 @@ AIE_DEV void stream_bits_f32(float *dst, int total, const uint32_t *bits, const 
     AIE_UNROLL(1)
     for (; g + 3 * NT < r.nq; g += 4 * NT) {
         const uint32_t v0 = b8[0], v1 = b8[hb], v2 = b8[2 * hb], v3 = b8[3 * hb];
-        q4[0] = lut4[(v0 >> sh) & 15u]; q4[NT] = lut4[(v1 >> sh) & 15u];
-        q4[2 * NT] = lut4[(v2 >> sh) & 15u]; q4[3 * NT] = lut4[(v3 >> sh) & 15u];
+        __stcs(q4, lut4[(v0 >> sh) & 15u]); __stcs(q4 + NT, lut4[(v1 >> sh) & 15u]);
+        __stcs(q4 + 2 * NT, lut4[(v2 >> sh) & 15u]); __stcs(q4 + 3 * NT, lut4[(v3 >> sh) & 15u]);
         b8 += 4 * hb; q4 += 4 * NT;
     }
     AIE_UNROLL(1)
-    for (; g < r.nq; g += NT) { q4[0] = lut4[((uint32_t)b8[0] >> sh) & 15u]; b8 += hb; q4 += NT; }
+    for (; g < r.nq; g += NT) { __stcs(q4, lut4[((uint32_t)b8[0] >> sh) & 15u]); b8 += hb; q4 += NT; }
 #else
     for (; g < r.nq; g += NT) {
         const uint32_t nib = ((uint32_t)b8[0] >> sh) & 15u;
