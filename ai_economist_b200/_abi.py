@@ -91,6 +91,10 @@ class AieFlatField(C.Structure):
     _fields_ = [("key", C.c_char * 64), ("offset", C.c_int32), ("size", C.c_int32)]
 
 
+class AieMetricKey(C.Structure):
+    _fields_ = [("key", C.c_char * 64), ("is_int", C.c_int32)]
+
+
 class AieField(C.Structure):
     _fields_ = [("offset", C.c_int32), ("elem_bytes", C.c_int32), ("is_float", C.c_int32),
                 ("is_signed", C.c_int32), ("ndim", C.c_int32), ("shape", C.c_int32 * 4)]
@@ -171,6 +175,10 @@ def load_library(path=None):
     L.aie_read_state.argtypes = [P, C.c_int32, C.POINTER(AieStateDump)]
     L.aie_read_episode_final.argtypes = [P, C.c_int32, C.POINTER(AieStateDump)]
     L.aie_read_episode_final.restype = C.c_int
+    L.aie_get_metric_layout.argtypes = [P, C.POINTER(AieMetricKey), C.c_int32]
+    L.aie_get_metric_layout.restype = C.c_int
+    L.aie_episode_metrics.argtypes = [P, C.c_int32, P, P]
+    L.aie_episode_metrics.restype = C.c_int
     L.aie_launch_count.argtypes = [P]
     L.aie_covid_create.argtypes = [C.POINTER(AieCovidConfig), C.c_int32, C.c_int32, C.POINTER(P)]
     L.aie_covid_destroy.argtypes = [P]
@@ -195,7 +203,8 @@ def load_library(path=None):
 
 EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field", "aie_get_flat_layout", "aie_bind_buffers",
                     "aie_load_state", "aie_step", "aie_step_dynamics", "aie_observe", "aie_sample_random_actions", "aie_set_fused_policy",
-                    "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final", "aie_launch_count", "aie_last_error", "aie_abi_version",
+                    "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
+                    "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
                     "aie_covid_sample_random_actions", "aie_covid_launch_count"]
 

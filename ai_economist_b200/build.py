@@ -5,7 +5,7 @@ import subprocess
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 LIB = os.path.join(CSRC, "libaie_b200.so")
 SOURCES = ["aie_abi.cu", "aie_expand_host.cpp"]
-DEPS = ["aie_abi.cu", "aie_expand_host.cpp", "aie_abi.inl", "aie_core.cuh", "aie_obs.cuh", "aie_host.h", "aie_layout.h", "aie_covid_core.cuh", "aie_covid_abi.inl", "aie_compact.cuh", "aie_compact_host.h",
+DEPS = ["aie_abi.cu", "aie_expand_host.cpp", "aie_abi.inl", "aie_core.cuh", "aie_obs.cuh", "aie_host.h", "aie_layout.h", "aie_covid_core.cuh", "aie_covid_abi.inl", "aie_compact.cuh", "aie_compact_host.h", "aie_metrics.cuh",
         "../../include/aie_b200.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
               "-shared", "-Xcompiler", "-fPIC"]

@@ -7,6 +7,7 @@
 //   aie_observe_kernel     one CTA per env replica.  Bulk-loads the observable prefix of the record and streams
 //                          out every observation / mask tensor with coalesced stores (the HBM-bound part).
 //   aie_finish_reset_kernel  one warp per env: tax trackers + utility metric_0 after a host reset upload.
+//   aie_metrics_kernel     one warp per env: env.metrics from the record in global memory, one row of a float64 table.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -18,6 +19,7 @@
 #include "aie_covid_core.cuh"
 #include "aie_host.h"
 #include "aie_compact.cuh"
+#include "aie_metrics.cuh"
 
 struct aie_env;
 struct aie_covid_env;
@@ -67,6 +69,7 @@ int launch_finish_reset(aie_env *, int lo, int n, void *stream);
 int launch_step(aie_env *, int emit_obs, void *stream);
 int launch_step_range(aie_env *, int emit_obs, int lo, int hi, void *stream);
 int launch_observe(aie_env *, int lo, int n, void *stream);
+int launch_metrics(aie_env *, int source, double *out, void *stream);
 int launch_sample(aie_env *, uint64_t seed, void *stream);
 int compact_buffers(aie_env *, size_t bytes, uint8_t **dev, uint8_t **host);
 int staging_node(aie_env *);
@@ -372,6 +375,17 @@ __global__ void __launch_bounds__(128, 4) aie_observe_mw_kernel(const __grid_con
     observe_env<EXT>(c, rec, grec, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<128, false>{(int)threadIdx.x});
 }
 
+// Episode metrics (aie_metrics.cuh): one warp per env, eight per CTA, reads the env's record (current or end-of-episode
+// snapshot) from global memory and writes row env of out [n_envs, K].
+__global__ void __launch_bounds__(256) aie_metrics_kernel(const __grid_constant__ DevCfg c, const uint8_t *recs, const uint32_t *prog,
+                                                          int K, int source, double *out) {
+    __shared__ double sm[8][MET_WARP_DOUBLES];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int env = blockIdx.x * 8 + warp;
+    if (env >= c.n_envs) return;
+    metrics_env(c, recs + (size_t)env * c.rec_bytes, prog, K, source, out + (size_t)env * K, sm[warp], lane);
+}
+
 // per_unit == 0: one warp per env (fastest for few agents: c2 15.2 us vs 17.5 us);  per_unit == 1: one warp per
 // (env, agent | planner bracket) - many agents x subspaces make the per-env chain long (c5: 64 agents x 6 subspaces).
 template <bool EXT>
@@ -648,6 +662,15 @@ int launch_observe(aie_env *env, int lo, int n, void *stream) {
     } else if (env->cfg.ext) aie_observe_kernel<true><<<(n + wpb - 1) / wpb, wpb * 32, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);
     else aie_observe_kernel<false><<<(n + wpb - 1) / wpb, wpb * 32, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);
     AIE_CUDA(cudaGetLastError(), "aie_observe_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+
+int launch_metrics(aie_env *env, int source, double *out, void *stream) {
+    const uint8_t *recs = source == 1 ? env->bufs.final : env->bufs.state;
+    aie_metrics_kernel<<<(env->n_envs + 7) / 8, 256, 0, (cudaStream_t)stream>>>(
+        env->cfg, recs, (const uint32_t *)env->metric_prog_dev, (int)env->metric_keys.size(), source, out);
+    AIE_CUDA(cudaGetLastError(), "aie_metrics_kernel launch");
     env->launches++;
     return AIE_OK;
 }

@@ -458,6 +458,87 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
     return AIE_OK;
 }
 
+// The columns of the episode-metrics table: the keys of the reference's env.metrics for this config in the dict's
+// insertion order (foundation/metrics.py builds the same dict), each with the MT_* op the metrics kernel evaluates there.
+// Scenario keys first, then every component's in component order; keys a config does not have are left out.
+inline void build_metric_layout(const DevCfg &c, std::vector<aie_metric_key> &keys, std::vector<uint32_t> &prog) {
+    keys.clear(); prog.clear();
+    auto add = [&](const std::string &k, int op, int arg, int is_int) {
+        aie_metric_key m;
+        memset(&m, 0, sizeof(m));
+        snprintf(m.key, sizeof(m.key), "%s", k.c_str());
+        m.is_int = is_int;
+        keys.push_back(m);
+        prog.push_back((uint32_t)op << 24 | (uint32_t)arg);
+    };
+    const int A = c.A;
+    auto num =[](int i) { return std::to_string(i); };
+    add("social/productivity", MT_PRODUCTIVITY, 0, 0);
+    add("social/equality", MT_EQUALITY, 0, 0);
+    add("social_welfare/coin_eq_times_productivity", MT_COIN_EQ_PROD, 0, 0);
+    if (c.one_step) {   // one_step_economy.py:210-262
+        add("social_welfare/inv_income_weighted_utility", MT_INV_W_UTIL, 0, 0);
+        add("endow/avg_agent/Coin", MT_MEAN_COIN, 0, 0);
+        add("endogenous/avg_agent/Labor", MT_MEAN_LABOR, 0, 0);
+        add("util/avg_agent", MT_MEAN_UTIL, 0, 0);
+        add("endow/p/Coin", MT_ZERO, 0, 1);
+        add("util/p", MT_UTIL, A, 0);
+    } else {            // layout_from_file.py:595-650
+        add("social_welfare/inv_income_weighted_coin_endow", MT_INV_W_COIN, 0, 0);
+        add("social_welfare/inv_income_weighted_utility", MT_INV_W_UTIL, 0, 0);
+        for (int a = 0; a < A; a++) {
+            add("endow/" + num(a) + "/Coin", MT_COIN, a, 0);
+            add("endow/" + num(a) + "/Stone", MT_INV, 2 * a, 0);
+            add("endow/" + num(a) + "/Wood", MT_INV, 2 * a + 1, 0);
+            add("endogenous/" + num(a) + "/Labor", MT_LABOR, a, 0);
+            add("util/" + num(a), MT_UTIL, a, 0);
+        }
+        for (const char *r : {"Coin", "Stone", "Wood"}) add(std::string("endow/p/") + r, MT_ZERO, 0, 0);
+        add("util/p", MT_UTIL, A, 0);
+        add("labor/weighted_cost", MT_WEIGHTED_COST, 0, 0);
+        add("labor/warmup_integrator", MT_WARMUP_INT, 0, 1);
+    }
+    static const char *CN[2] = {"Stone", "Wood"}, *SIDE[2] = {"Sell", "Buy"};
+    for (int i = 0; i < c.n_comp; i++) {
+        if (c.comp[i] == COMP_BUILD) {   // build.py:198-222
+            for (int a = 0; a < A; a++) add("Build/" + num(a) + "/n_builds", MT_N_BUILDS, a, 1);
+            add("Build/total_builds", MT_TOTAL_BUILDS, 0, 1);
+        } else if (c.comp[i] == COMP_CDA) {   // continuous_double_auction.py:585-641 (cost == income == price)
+            for (int a = 0; a < A; a++)
+                for (int cc = 0; cc < 2; cc++)
+                    for (int side = 0; side < 2; side++) {
+                        const std::string p = "Trade/" + num(a) + "/" + SIDE[side] + CN[cc] + "/";
+                        const int idx = c.st_trade + ((a * 2 + cc) * 2 + side) * 2;
+                        for (const char *k : {"price", "cost", "income"}) add(p + k, MT_TRADE_AVG, idx, 0);
+                        add(p + "n_sales", MT_TRADE_N, idx, 1);
+                    }
+            add("Trade/n_trades", MT_N_TRADES, 0, 1);
+        } else if (c.comp[i] == COMP_TAX) {   // redistribution.py:1141-1186
+            // the reference keys its logs by "%03d" % int(cutoff): brackets that share a key are pooled, in first-seen order
+            std::vector<std::pair<std::string, int>> groups;
+            for (int b = 0; b < c.B; b++) {
+                char k[32];
+                snprintf(k, sizeof(k), "%03lld", (long long)c.cutoffs[b]);
+                auto it = std::find_if(groups.begin(), groups.end(), [&](const std::pair<std::string, int> &g) { return g.first == k; });
+                if (it == groups.end()) groups.push_back({k, 1 << b});
+                else it->second |= 1 << b;
+            }
+            for (const auto &g : groups) {
+                add("PeriodicTax/avg_bracket_rate/" + g.first, MT_BRACKET_RATE, g.second, 0);
+                add("PeriodicTax/bracket_occupancy/" + g.first, MT_BRACKET_OCC, g.second, 0);
+            }
+            if (!c.disable_taxes) {
+                add("PeriodicTax/avg_effective_tax_rate", MT_EFF_RATE, 0, 0);
+                add("PeriodicTax/total_collected_taxes", MT_COLLECTED, 0, 0);
+                add("PeriodicTax/avg_tax_rate/poorest", MT_TAX_POOREST, 0, 0);
+                add("PeriodicTax/avg_tax_rate/richest", MT_TAX_RICHEST, 0, 0);
+                // the running elasticity estimate lives in the host-side Saez estimator: the caller fills this column
+                if (c.tax_model == AIE_TAX_SAEZ) add("PeriodicTax/saez/estimated_elasticity", MT_NAN, 0, 0);
+            }
+        }
+    }
+}
+
 inline void fill_dims(const DevCfg &c, aie_dims &d) {
     memset(&d, 0, sizeof(d));
     d.n_envs = c.n_envs; d.n_agents = c.A; d.height = c.H; d.width = c.W;

@@ -45,6 +45,15 @@ enum { ST_TAX_PERIODS = 0, ST_TAX_COLLECTED = 1, ST_TAX_EFF_SUM = 2, ST_TAX_SCHE
 //   EV_TRADE  {kind, seller, buyer, commodity, ask, bid, ask_lifetime, bid_lifetime}
 enum { EV_BUILD = 1, EV_GATHER = 2, EV_TRADE = 3 };
 
+// Episode metrics (aie_metrics.cuh): one op word per column of the [E, K] table, op << 24 | argument.  The host builds
+// the program with the key names (aie_host.h: build_metric_layout).  Arguments: MT_COIN / MT_LABOR / MT_N_BUILDS agent a;
+// MT_UTIL agent a (a == A: planner); MT_INV 2a + resource (0 Stone, 1 Wood); MT_TRADE_AVG / MT_TRADE_N the stats index of
+// the (count, price sum) pair; MT_BRACKET_RATE / MT_BRACKET_OCC the bitmask of the brackets pooled under one key.
+enum { MT_NAN = 0, MT_ZERO, MT_PRODUCTIVITY, MT_EQUALITY, MT_COIN_EQ_PROD, MT_INV_W_COIN, MT_INV_W_UTIL, MT_MEAN_COIN,
+       MT_MEAN_LABOR, MT_MEAN_UTIL, MT_COIN, MT_INV, MT_LABOR, MT_UTIL, MT_WEIGHTED_COST, MT_WARMUP_INT, MT_N_BUILDS,
+       MT_TOTAL_BUILDS, MT_TRADE_AVG, MT_TRADE_N, MT_N_TRADES, MT_BRACKET_RATE, MT_BRACKET_OCC, MT_EFF_RATE, MT_COLLECTED,
+       MT_TAX_POOREST, MT_TAX_RICHEST };
+
 enum { COMP_BUILD = 0, COMP_CDA = 1, COMP_GATHER = 2, COMP_TAX = 3, COMP_WEALTH = 4, COMP_LABOR = 5, COMP_KINDS = 6 };
 enum { SUB_BUILD = 0, SUB_BUY = 1, SUB_SELL = 2, SUB_GATHER = 3, SUB_LABOR = 4 };
 

@@ -637,3 +637,61 @@ class BatchedFoundationEnv:
             return None
         return metrics_from_state(self._spec, fin, saez_elasticity=self._saez.elas_at_episode_end[e]
                                   if self._saez is not None else None)
+
+    # ------------------------------------------------------------------ batched metrics (one launch for every replica)
+    @property
+    def metric_keys(self):
+        """Column order of metrics_tensor() / previous_episode_metrics_tensor(): the keys of metrics_of(e), in order."""
+        return [k for k, _ in self._stepper.metric_layout()]
+
+    def metrics_tensor(self, out=None):
+        """`env.metrics` of every replica as one float64 tensor [n_envs, K] on the device (columns: metric_keys), computed
+        by one kernel launch with no synchronisation and no host copy; row e equals metrics_of(e).  A training loop reads
+        the curves it logs (productivity, equality, trades, tax rates) without stalling the stream, e.g.
+        `env.metrics_tensor()[:, env.metric_keys.index("social/productivity")].mean()`.  out: an optional preallocated
+        contiguous float64 [n_envs, K] tensor."""
+        m = self._stepper.episode_metrics(final=False, out=out)
+        if self._saez is not None:
+            self._fill_saez_elasticity(m, np.asarray(self._saez.batch.elas_tm1, np.float64))
+        return m
+
+    def previous_episode_metrics_tensor(self, out=None):
+        """previous_episode_metrics of every replica as one float64 tensor [n_envs, K] (columns: metric_keys): the
+        metrics of the episode each replica finished last, NaN in every column for a replica that has finished none.
+        Needs auto_reset (the end-of-episode records); without it the library's AieError is raised.  Training-loop idiom,
+        the metrics of the episodes that ended in this step with no synchronisation until the caller reduces them:
+            m = env.previous_episode_metrics_tensor(); logged = m[env.done["__all__"].bool()]"""
+        m = self._stepper.episode_metrics(final=True, out=out)
+        if self._saez is not None:
+            ends = self._saez.elas_at_episode_end
+            self._fill_saez_elasticity(m, np.array([np.nan if v is None else v for v in ends], np.float64), keep_nan_rows=True)
+        return m
+
+    def _fill_saez_elasticity(self, m, values, keep_nan_rows=False):
+        """The Saez estimator runs on the host: its elasticity column is filled with one host-to-device copy of E doubles.
+        keep_nan_rows: rows the device wrote as all NaN (no finished episode) stay NaN."""
+        keys = self.metric_keys
+        col = keys.index("PeriodicTax/saez/estimated_elasticity")
+        if isinstance(m, np.ndarray):
+            m[:, col] = np.where(np.isnan(m[:, 0]), np.nan, values) if keep_nan_rows else values
+            return
+        import torch
+        v = torch.as_tensor(values).to(m.device)
+        m[:, col] = torch.where(torch.isnan(m[:, 0]), m[:, col], v) if keep_nan_rows else v
+
+    def metrics_rows_as_dicts(self, rows, envs=None):
+        """Rows of metrics_tensor() / previous_episode_metrics_tensor() ([n, K], tensor or array) back as the dicts
+        metrics_of(e) / previous_episode_metrics_of(e) return: same key order, ints as int, NaN as float("nan"); a row
+        that is NaN in every column (no finished episode yet) becomes None.  envs: the row indices to convert (default:
+        all).  Copies the rows to the host, i.e. synchronises with the stream that produced them."""
+        a = rows.detach().cpu().numpy() if hasattr(rows, "detach") else np.asarray(rows)
+        a = np.asarray(a, np.float64).reshape(-1, a.shape[-1])
+        layout = self._stepper.metric_layout()
+        out = []
+        for e in (range(a.shape[0]) if envs is None else envs):
+            r = a[int(e)]
+            if np.isnan(r).all():
+                out.append(None)
+                continue
+            out.append({k: (int(v) if is_int else float(v)) for (k, is_int), v in zip(layout, r.tolist())})
+        return out

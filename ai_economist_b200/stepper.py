@@ -80,6 +80,10 @@ class BatchStepper:
     def _stream(self):
         return None
 
+    def _empty(self, shape, dt):
+        """An output buffer whose contents are about to be overwritten (default: the zeroed allocation)."""
+        return self._alloc(shape, dt)
+
     def to_numpy(self, buf):
         raise NotImplementedError
 
@@ -109,6 +113,34 @@ class BatchStepper:
         arr = (_abi.AieFlatField * max(1, n))()
         self.lib.aie_get_flat_layout(self._h, idx, arr, n)
         return [(arr[i].key.decode(), int(arr[i].offset), int(arr[i].size)) for i in range(n)]
+
+    def metric_layout(self):
+        """[(key, is_int)] of the episode-metrics table's columns: the reference's env.metrics keys for this config in
+        their dict order (aie_get_metric_layout)."""
+        if getattr(self, "_metric_layout", None) is None:
+            n = self.lib.aie_get_metric_layout(self._h, None, 0)
+            if n < 0:
+                self._check(n)
+            arr = (_abi.AieMetricKey * max(1, n))()
+            self.lib.aie_get_metric_layout(self._h, arr, n)
+            self._metric_layout = [(arr[i].key.decode(), bool(arr[i].is_int)) for i in range(n)]
+        return list(self._metric_layout)
+
+    def episode_metrics(self, final=False, out=None):
+        """env.metrics of every replica as a float64 table [n_envs, K] in metric_layout() order, computed on the device by
+        one kernel launch, asynchronous on the stream (aie_episode_metrics).  final=True: the metrics of each replica's
+        last finished episode (needs auto_reset; rows of replicas that have finished none are NaN).  out: an optional
+        preallocated contiguous float64 [n_envs, K] buffer on the same device."""
+        K = len(self.metric_layout())
+        if out is None:
+            out = self._empty((self.n_envs, K), "f64")
+        elif tuple(out.shape) != (self.n_envs, K) or not self._is_f64_contiguous(out):
+            raise _abi.AieError("episode_metrics: out must be a contiguous float64 [%d, %d] buffer" % (self.n_envs, K))
+        self._check(self.lib.aie_episode_metrics(self._h, 1 if final else 0, self._ptr(out), self._stream()))
+        return out
+
+    def _is_f64_contiguous(self, buf):
+        return isinstance(buf, np.ndarray) and buf.dtype == np.float64 and buf.flags["C_CONTIGUOUS"]
 
     def load_state(self, host_state, env_lo=0):
         """host_state: dict of numpy arrays with a leading env axis (see aie_host_state in the header)."""
@@ -266,6 +298,15 @@ class CudaStepper(BatchStepper):
         t = self.torch
         m = {"u8": t.uint8, "i16": t.int16, "i32": t.int32, "f32": t.float32, "f64": t.float64}
         return t.zeros(shape, dtype=m[dt], device=self.device)
+
+    def _empty(self, shape, dt):
+        t = self.torch
+        m = {"u8": t.uint8, "i16": t.int16, "i32": t.int32, "f32": t.float32, "f64": t.float64}
+        return t.empty(shape, dtype=m[dt], device=self.device)
+
+    def _is_f64_contiguous(self, buf):
+        t = self.torch
+        return isinstance(buf, t.Tensor) and buf.dtype == t.float64 and buf.is_contiguous() and buf.device == self.device
 
     def _ptr(self, buf):
         return C.c_void_p(buf.data_ptr())

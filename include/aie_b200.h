@@ -376,6 +376,23 @@ int aie_read_state(aie_env *env, int32_t e, const aie_state_dump *out);
  * not part of the snapshot (book_rows / book_count are ignored).  AIE_ESTATE when no episode_final buffer is bound. */
 int aie_read_episode_final(aie_env *env, int32_t env_index, const aie_state_dump *out);
 
+/* Episode metrics of every replica in one launch (aie_metrics_kernel: one warp per env reads its record in global
+ * memory and writes one row).  Each row is BaseEnvironment.metrics (base_env.py:421-432) of that replica, i.e. what
+ * foundation/metrics.py computes from one record, summed in numpy's order.
+ *
+ * The reference's env.metrics keys for this config, in column order; is_int marks keys whose reference value is an
+ * int (n_builds, total_builds, n_sales, n_trades, warmup_integrator, one-step "endow/p/Coin").  Fills at most cap
+ * entries, returns K (or a negative AIE_E* code), like aie_get_flat_layout. */
+typedef struct aie_metric_key { char key[64]; int32_t is_int; } aie_metric_key;
+int aie_get_metric_layout(const aie_env *env, aie_metric_key *out, int32_t cap);
+/* source 0: the current records (env.metrics of every replica; a replica at t >= episode_length counts its finished
+ * episode, like the reference before its reset); 1: the episode_final records (previous_episode_metrics; a replica that
+ * has finished no episode yet gets a row of NaN).  out: DEVICE float64 [n_envs, K].  Asynchronous on `stream`: no
+ * synchronisation, no host copy.  Trade averages without trades are NaN; the Saez model's estimated_elasticity column
+ * is written NaN (the estimator runs on the host).  AIE_EINVAL for a NULL out or an unknown source, AIE_ESTATE before
+ * aie_bind_buffers or, for source 1, without an episode_final buffer. */
+int aie_episode_metrics(aie_env *env, int32_t source, double *out, void *stream);
+
 /* Number of kernels the library has launched on this handle since creation (for bench "gpu_launches"). */
 int64_t aie_launch_count(const aie_env *env);
 
