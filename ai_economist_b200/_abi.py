@@ -76,6 +76,10 @@ class AieHostState(C.Structure):
         "build_payment", "build_skill", "bonus_gather_prob", "mt_key", "mt_pos", "completions", "gauss_has", "gauss_val", "split_skill"]]
 
 
+class AieResetStreams(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ["mt_key", "mt_pos", "gauss_has", "gauss_val", "split_skill"]]
+
+
 _DUMP_PTRS = ["cell", "owner", "loc", "coin", "esc_coin", "labor", "inv", "esc", "n_orders", "bid_hist", "ask_hist",
               "price_hist", "tax_pos", "rate_idx", "last_coin", "last_income", "last_marg", "mt_key", "mt_pos", "t",
               "completions", "book_rows", "book_count"]
@@ -160,6 +164,8 @@ def load_library(path=None):
     L.aie_get_flat_layout.restype = C.c_int
     L.aie_bind_buffers.argtypes = [P, C.POINTER(AieBuffers)]
     L.aie_load_state.argtypes = [P, C.POINTER(AieHostState), C.c_int32, P]
+    L.aie_reset_envs.argtypes = [P, C.POINTER(AieHostState), C.POINTER(AieResetStreams), C.c_int32, C.c_int32, P]
+    L.aie_reset_envs.restype = C.c_int
     L.aie_step.argtypes = [P, P]
     L.aie_observe.argtypes = [P, P]
     L.aie_step_dynamics.argtypes = [P, P]
@@ -202,7 +208,7 @@ def load_library(path=None):
 
 
 EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field", "aie_get_flat_layout", "aie_bind_buffers",
-                    "aie_load_state", "aie_step", "aie_step_dynamics", "aie_observe", "aie_sample_random_actions", "aie_set_fused_policy",
+                    "aie_load_state", "aie_reset_envs", "aie_step", "aie_step_dynamics", "aie_observe", "aie_sample_random_actions", "aie_set_fused_policy",
                     "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
                     "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",

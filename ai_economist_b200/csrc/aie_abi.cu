@@ -7,6 +7,7 @@
 //   aie_observe_kernel     one CTA per env replica.  Bulk-loads the observable prefix of the record and streams
 //                          out every observation / mask tensor with coalesced stores (the HBM-bound part).
 //   aie_finish_reset_kernel  one warp per env: tax trackers + utility metric_0 after a host reset upload.
+//   aie_reset_kernel       one warp per env: explicit reset on the device (aie_reset_envs), the auto-reset's re-draws.
 //   aie_metrics_kernel     one warp per env: env.metrics from the record in global memory, one row of a float64 table.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -66,6 +67,7 @@ int dev_copy(aie_env *, void *dst, const void *src, size_t n, void *stream);
 int sync(aie_env *, void *stream);
 int sync_all(aie_env *);
 int launch_finish_reset(aie_env *, int lo, int n, void *stream);
+int launch_reset(aie_env *, const ResetSrc &s, int lo, int n, void *stream);
 int launch_step(aie_env *, int emit_obs, void *stream);
 int launch_step_range(aie_env *, int emit_obs, int lo, int hi, void *stream);
 int launch_observe(aie_env *, int lo, int n, void *stream);
@@ -329,6 +331,69 @@ __global__ void __launch_bounds__(256) aie_finish_reset_kernel(const __grid_cons
     }
 }
 
+// Explicit reset on the device (aie_reset_envs, reset_mode == 1): one warp per env, up to step_wpb envs per CTA, or one
+// CTA per env for large records (the reset is serial per env: one warp).  The record is restored from the template or
+// the env's state0, gets its stream and header, and is re-drawn as the auto-reset re-draws it; the result is what
+// aie_load_state leaves for the host reset of the same stream.  The observations follow in aie_observe_kernel.
+template <bool EXT>
+__global__ void __launch_bounds__(256) aie_reset_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
+                                                        const ResetSrc s, int lo, int n) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int wpb = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * wpb + warp;
+    if (i >= n) return;
+    const int env = lo + i;
+    uint64_t *bar = (uint64_t *)smem + warp;
+    uint8_t *rec = warp_region(smem, wpb, warp, c);
+    uint8_t *scratch = rec + c.resident_bytes;
+    uint8_t *grec = b.state + (size_t)env * c.rec_bytes, *snap = b.state0 + (size_t)env * c.rec_bytes;
+    const uint8_t *src = s.tmpl ? s.tmpl : snap;
+    // counters of the current record (an episode that has ended and waits for this reset counts as completed), read
+    // before anything is written
+    const int32_t *cur = (const int32_t *)grec;
+    const int32_t completions = s.counters_from_record ? cur[HDR_COMPLETIONS] + (cur[HDR_T] >= c.T ? 1 : 0)
+                                                       : ((const int32_t *)src)[HDR_COMPLETIONS];
+    const int32_t warm = s.counters_from_record ? cur[HDR_AUTO_WARMUP] : 0;
+    const int32_t mt_pos = s.mt_key ? s.mt_pos[i] : cur[HDR_MT_POS];
+    const uint32_t tail = (uint32_t)(c.rec_bytes - c.off_price_hist);  // price history + order slots (+ split statistics)
+    __syncwarp();
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        mbar_expect_tx(bar, (uint32_t)c.off_mt + (c.split ? 0u : tail) + (s.mt_key ? 0u : (uint32_t)c.keep_bytes));
+        bulk_g2s(rec, src, (uint32_t)c.off_mt, bar);
+        if (!c.split) bulk_g2s(rec + c.off_price_hist, src + c.off_price_hist, tail, bar);
+        if (!s.mt_key) bulk_g2s(rec + c.off_mt, grec + c.off_mt, (uint32_t)c.keep_bytes, bar);
+    }
+    if (c.split) {  // the big sections live in global memory: plain copies
+        const uint4 *from = (const uint4 *)(src + c.off_price_hist);
+        uint4 *to = (uint4 *)(grec + c.off_price_hist);
+        for (uint32_t k = lane; k < tail / 16; k += 32) to[k] = from[k];
+    }
+    __syncwarp();
+    mbar_wait(bar, 0);
+    reset_install_stream(c, s, i, rec, completions, mt_pos, lane);
+    device_reset_env<EXT>(c, rec, grec, scratch, lane, b.dyn_prob, b.dyn_work ? b.dyn_work + (size_t)env * (c.HW + 16) : nullptr);
+    finish_reset_env(c, rec, grec, scratch, lane);
+    if (lane == 0) b.done[env] = 0;
+    for (int a = lane; a <= c.A; a += 32) b.rew[(size_t)env * (c.A + 1) + a] = 0.0;
+    if (c.split) {  // state0 gets the same big sections
+        const uint4 *from = (const uint4 *)(grec + c.off_price_hist);
+        uint4 *to = (uint4 *)(snap + c.off_price_hist);
+        for (uint32_t k = lane; k < tail / 16; k += 32) to[k] = from[k];
+    }
+    fence_async_smem();
+    __syncwarp();
+    // state0 as aie_load_state leaves it (auto_warmup 0); the live record carries the warm-up integrator over
+    if (lane == 0) {
+        bulk_s2g(snap, rec, (uint32_t)c.resident_bytes);
+        bulk_wait_read();
+        ((int32_t *)rec)[HDR_AUTO_WARMUP] = warm;
+        fence_async_smem();
+        bulk_s2g(grec, rec, (uint32_t)c.resident_bytes);
+        bulk_wait_read();
+    }
+}
+
 // Stand-alone observation pass (after a reset upload, or when the caller steps dynamics separately): bulk-loads only
 // what observe_env reads.  One warp per env, or (MW) one CTA of four warps per env.
 // observe_env reads the record's prefix [0, obs_prefix_bytes) and, outside it, only in phase A (before any staging
@@ -483,6 +548,7 @@ int init(aie_env *env) {
     AIE_OPT_IN((aie_step_mw_kernel<false, false>)); AIE_OPT_IN((aie_step_mw_kernel<false, true>));
     AIE_OPT_IN((aie_step_mw_kernel<true, false>)); AIE_OPT_IN((aie_step_mw_kernel<true, true>));
     AIE_OPT_IN(aie_finish_reset_kernel);
+    AIE_OPT_IN(aie_reset_kernel<false>); AIE_OPT_IN(aie_reset_kernel<true>);
     AIE_OPT_IN(aie_observe_kernel<false>); AIE_OPT_IN(aie_observe_kernel<true>);
     AIE_OPT_IN(aie_observe_mw_kernel<false>); AIE_OPT_IN(aie_observe_mw_kernel<true>);
 #undef AIE_OPT_IN
@@ -615,6 +681,16 @@ int launch_finish_reset(aie_env *env, int lo, int n, void *stream) {
     const int wpb = env->be.step_wpb;
     aie_finish_reset_kernel<<<(n + wpb - 1) / wpb, wpb * 32, env->be.step_smem, (cudaStream_t)stream>>>(env->cfg, env->bufs, lo, n);
     AIE_CUDA(cudaGetLastError(), "aie_finish_reset_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+int launch_reset(aie_env *env, const ResetSrc &s, int lo, int n, void *stream) {
+    const int wpb = env->be.step_wpb;   // as the step kernel's shared memory: 1 when mw > 1 (one CTA, one warp per env)
+    const dim3 grid((n + wpb - 1) / wpb), block(32 * wpb);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (env->cfg.ext) aie_reset_kernel<true><<<grid, block, env->be.step_smem, st>>>(env->cfg, env->bufs, s, lo, n);
+    else aie_reset_kernel<false><<<grid, block, env->be.step_smem, st>>>(env->cfg, env->bufs, s, lo, n);
+    AIE_CUDA(cudaGetLastError(), "aie_reset_kernel launch");
     env->launches++;
     return AIE_OK;
 }

@@ -1480,6 +1480,34 @@ AIE_DEV_NOINLINE void device_reset_env(const DevCfg &c, uint8_t *rec, uint8_t *g
     wsync();
 }
 
+// Explicit reset (aie_reset_envs), after env i's record image [0, off_mt) (and the big sections) has been restored from
+// the template or state0 and, without new streams, the kept section [off_mt, off_mt + keep_bytes) loaded from the current
+// record: the header and kept section a host reset packs (aie_host.h: pack_record) - counters zero but completions, the
+// stream installed, the Saez section zeroed (the caller's Saez estimator writes its persistent state back afterwards).
+AIE_DEV void reset_install_stream(const DevCfg &c, const ResetSrc &s, int i, uint8_t *rec, int32_t completions,
+                                  int32_t mt_pos, int lane) {
+    if (s.mt_key) {
+        uint32_t *kept = (uint32_t *)(rec + c.off_mt);
+        for (int k = lane; k < c.keep_bytes / 4; k += NL) kept[k] = 0u;
+        wsync();
+        for (int k = lane; k < 624; k += NL) kept[k] = s.mt_key[(size_t)i * 624 + k];
+        if (c.off_gauss && lane == 0) {
+            double *g = (double *)(rec + c.off_gauss);
+            g[0] = s.gauss[2 * (size_t)i]; g[1] = s.gauss[2 * (size_t)i + 1];
+        }
+        if (c.off_split_skill)
+            for (int a = lane; a < c.A; a += NL) ((double *)(rec + c.off_split_skill))[a] = s.split_skill[(size_t)i * c.A + a];
+    } else if (c.off_saez) {
+        for (int k = lane; k < 48; k += NL) ((double *)(rec + c.off_saez))[k] = 0.0;
+    }
+    if (lane == 0) {
+        int32_t *hdr = (int32_t *)rec;
+        for (int w = 0; w < HDR_WORDS; w++) hdr[w] = 0;
+        hdr[HDR_TAX_POS] = 1; hdr[HDR_COMPLETIONS] = completions; hdr[HDR_MT_POS] = mt_pos;
+    }
+    wsync();
+}
+
 }  // namespace aie
 
 #include "aie_obs.cuh"   // observations + masks (the other half of the fused step kernel)

@@ -189,6 +189,17 @@ struct DevBufs {
     // into the action buffers, from the mask limits it has just staged - instead of a separate sampler launch per step
     uint64_t policy_seed;
 };
+
+// Explicit device-side reset (aie_reset_envs): where env i of the launched range takes its starting record and its numpy
+// stream from.  Device pointers, library-owned staging.
+struct ResetSrc {
+    const uint8_t *tmpl;          // one packed host-reset record for every env, or null: the env's own state0
+    const uint32_t *mt_key;       // [n][624] stream of env i, or null: the stream in the env's record continues
+    const int32_t *mt_pos;        // [n]
+    const double *gauss;          // [n][2] {cached value, has}: records with a Gaussian cache (off_gauss)
+    const double *split_skill;    // [n][A] split_layout's rank -> payment table
+    int32_t counters_from_record; // 1: completions / auto_warmup come from the current record, 0: from tmpl
+};
 // compact program table: [agent flat (Fa) | planner flat (Fp) | p<i> flat (Fpa) | agent mask (Na)], offsets in DevCfg
 // then: histogram offsets u16 [4P <= 128], mask segments u16 [<= 64], nibble -> float4 table (64 floats = 128 u16)
 constexpr int TAB_WORDS = 2 * MAX_FLAT + 16 + MAX_MASK + 128 + 64 + 128 + 16 + MAX_FLAT;

@@ -370,6 +370,8 @@ class BatchedFoundationEnv:
             # base_env.py:763-765, 1022-1025: _finalize_logs stores the metrics only on the step that ENDS an episode, so
             # resetting an unfinished episode (or resetting twice) leaves previous_episode_metrics untouched
             self._last_ep_metrics_host = self.metrics_of(0, _count_finished=False)
+        if self._spec.get("reset_mode", 0) == 1 and hasattr(self._stepper, "reset_envs"):
+            return self._reset_on_device(seed_state, force_dense_logging)
         if self._loaded and self._rs is not None:
             self._completions = self.completions()
             self._sync_streams_from_device()
@@ -399,6 +401,59 @@ class BatchedFoundationEnv:
             self._saez.after_host_reset(saez_n)
         self._start_dense_log(force_dense_logging, int(self._completions[0]))
         return self.obs
+
+    def _reset_on_device(self, seed_state, force_dense_logging):
+        """reset() of a config whose auto-reset is reference-exact: one launch re-draws every replica on the device from
+        its own stream (aie_reset_envs) and leaves what the host reset of the same streams would.  Once loaded, nothing of
+        size n_envs crosses PCIe (Saez and dense logs aside): the streams, the completion counts and the energy warm-up
+        integrators stay in the records, as they do across an auto-reset."""
+        if seed_state is not None:
+            if self._rs is None:
+                self._rs = [np.random.RandomState() for _ in range(self.n_envs)]
+            per_env = seed_state if (isinstance(seed_state, (tuple, list)) and len(seed_state) == self.n_envs
+                                     and isinstance(seed_state[0], (tuple, list))) else [seed_state]
+            for e, ss in enumerate(per_env):
+                self.set_stream_state(ss, e)   # once loaded, this also installs the stream in replica e's record
+        saez_n = self._saez.before_host_reset() if self._saez is not None else None
+        if self._loaded:
+            self._stepper.reset_envs()
+        else:
+            streams = self._host_streams()
+            self._stepper.reset_envs(template=self._reset_template(), streams=streams)
+            self._loaded = True
+        if self._saez is not None:
+            self._saez.after_host_reset(saez_n)
+        completions0 = 0
+        if force_dense_logging or self._create_dense_log_every is not None:
+            st = self._stepper
+            completions0 = int(st.to_numpy(st.state_view("completions")[0:1])[0])
+        self._start_dense_log(force_dense_logging, completions0)
+        return self.obs
+
+    def _host_streams(self):
+        """Every replica's host stream (after the constructor's draws) in aie_reset_streams' layout."""
+        if self._rs is None:
+            self._rs = [np.random.RandomState() for _ in range(self.n_envs)]
+        states = [rs.get_state() for rs in self._rs]
+        out = dict(mt_key=np.stack([np.asarray(s[1], np.uint32) for s in states]),
+                   mt_pos=np.array([s[2] for s in states], np.int32),
+                   gauss_has=np.array([s[3] for s in states], np.int32),
+                   gauss_val=np.array([s[4] for s in states], np.float64))
+        out.update(self.scenario.device_reset_tables())
+        return out
+
+    def _reset_template(self):
+        """The host reset of replica 0 on a copy of its stream, as a one-replica snapshot: the parts of a starting
+        record that do not depend on the stream (maps of a fixed layout, coin, water) for every replica; the device
+        re-draws the rest."""
+        rs = np.random.RandomState()
+        rs.set_state(self._rs[0].get_state())
+        st = self.scenario.host_reset(rs, 0)
+        key = rs.get_state()
+        st["mt_key"], st["mt_pos"] = np.asarray(key[1], np.uint32), int(key[2])
+        st["gauss_has"], st["gauss_val"] = int(key[3]), float(key[4])
+        st["completions"] = int(self._completions[0])
+        return {k: np.asarray(v)[None] for k, v in st.items()}
 
     def _episode_finished(self, e):
         st = self._stepper

@@ -77,6 +77,10 @@ class BaseScenario:
             elif comp.name == "Gather":
                 st["bonus_gather_prob"] = comp.sample_skills(rs, A)
 
+    def device_reset_tables(self):
+        """Per-replica tables a device-side reset hands out again, besides the stream: {name: array [n_envs, ...]}."""
+        return {}
+
     def scenario_spec_fields(self):
         return dict(
             obs_range=self.obs_range, planner_gets_spatial_info=int(self.planner_gets_spatial_info),
@@ -475,6 +479,9 @@ class SplitLayout(LayoutFromFile):
         st["loc"] = loc
         st["split_skill"] = self._split_ranked_skill[e].copy()   # the device-side reset hands these out again
         return st
+
+    def device_reset_tables(self):
+        return {"split_skill": self._split_ranked_skill}
 
     def scenario_spec_fields(self):
         d = super().scenario_spec_fields()   # reset_mode 1 when the skill distributions have a device-side sampler

@@ -142,11 +142,8 @@ class BatchStepper:
     def _is_f64_contiguous(self, buf):
         return isinstance(buf, np.ndarray) and buf.dtype == np.float64 and buf.flags["C_CONTIGUOUS"]
 
-    def load_state(self, host_state, env_lo=0):
-        """host_state: dict of numpy arrays with a leading env axis (see aie_host_state in the header)."""
-        n = int(np.asarray(host_state["loc"]).shape[0])
-        keep = []
-
+    def _host_state(self, host_state, keep):
+        """aie_host_state over the numpy arrays of host_state (kept alive in `keep`)."""
         def arr(key, dt, required=True):
             v = host_state.get(key)
             if v is None:
@@ -157,7 +154,7 @@ class BatchStepper:
             return a.ctypes.data_as(C.c_void_p)
 
         hs = _abi.AieHostState()
-        hs.n = n
+        hs.n = int(np.asarray(host_state["loc"]).shape[0])
         for key, dt, req in [("stone", np.uint8, True), ("wood", np.uint8, True), ("stone_src", np.uint8, True),
                              ("wood_src", np.uint8, True), ("water", np.uint8, False), ("loc", np.int16, True),
                              ("coin", np.float64, True), ("inv_stone", np.int32, False), ("inv_wood", np.int32, False),
@@ -167,7 +164,35 @@ class BatchStepper:
                              ("gauss_has", np.int32, False), ("gauss_val", np.float64, False),
                              ("split_skill", np.float64, False)]:
             setattr(hs, key, arr(key, dt, req))
+        return hs
+
+    def load_state(self, host_state, env_lo=0):
+        """host_state: dict of numpy arrays with a leading env axis (see aie_host_state in the header)."""
+        keep = []
+        hs = self._host_state(host_state, keep)
         self._check(self.lib.aie_load_state(self._h, C.byref(hs), int(env_lo), self._stream()))
+
+    def reset_envs(self, template=None, streams=None, env_lo=0, n=None):
+        """Explicit reset of replicas [env_lo, env_lo + n) on the device (aie_reset_envs; configs with reset_mode == 1):
+        the records come out as load_state leaves them for the host reset of the same streams.  template: None (each
+        replica restarts from its own state0) or a host reset snapshot of ONE replica (load_state's dict, leading axis 1).
+        streams: None (each record's stream continues) or a dict of numpy arrays with a leading axis n: mt_key, mt_pos
+        and, where the config needs them, gauss_has / gauss_val, split_skill.  Asynchronous on the stream when neither is
+        given."""
+        n = self.n_envs - int(env_lo) if n is None else int(n)
+        keep = []
+        tmpl = C.byref(self._host_state(template, keep)) if template is not None else None
+        rs = None
+        if streams is not None:
+            s = _abi.AieResetStreams()
+            for key, dt in [("mt_key", np.uint32), ("mt_pos", np.int32), ("gauss_has", np.int32), ("gauss_val", np.float64),
+                            ("split_skill", np.float64)]:
+                if streams.get(key) is not None:
+                    a = np.ascontiguousarray(streams[key], dtype=dt)
+                    keep.append(a)
+                    setattr(s, key, a.ctypes.data_as(C.c_void_p))
+            rs = C.byref(s)
+        self._check(self.lib.aie_reset_envs(self._h, tmpl, rs, int(env_lo), n, self._stream()))
 
     def step(self):
         """Advance every env by one timestep from the bound action buffers (asynchronous on the stream)."""

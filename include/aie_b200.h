@@ -316,6 +316,31 @@ int aie_bind_buffers(aie_env *env, const aie_buffers *bufs);
  * writes their first observations/masks.  Synchronous. */
 int aie_load_state(aie_env *env, const aie_host_state *hs, int32_t env_lo, void *stream);
 
+/* Explicit reset on the device (configs with reset_mode == 1): env.reset() of replicas [env_lo, env_lo + n) without a
+ * host reset per replica.  One launch re-draws, from each replica's own numpy stream and in the reference's order, what
+ * the auto-reset re-draws (layout, placement, skills, fixed_four / split_layout assignment), then one launch writes the
+ * first observations.  Each record comes out as aie_load_state leaves it for the host reset of the same stream (byte
+ * for byte, except that the device's exp / log can move Pareto / lognormal skills and the cached Gaussian in the last place): t 0, episodes 0, Saez section and counter zero (the caller's Saez estimator restores them), reward and done
+ * zero, state0 the same record; the live record additionally carries auto_warmup over.  episode_final and the event
+ * log are not touched.
+ *   tmpl:    NULL: every replica restarts from its own state0 (the record its last reset produced).  Else one host reset
+ *            snapshot (n == 1): its maps, coin and inventories become every replica's starting record (everything
+ *            random in it is re-drawn); its completions count seeds replicas that have never been loaded.
+ *   streams: NULL: each record's stream continues.  Else the streams of the n replicas (arrays indexed from 0).
+ * Counters: once the env is loaded, completions = the record's count + 1 if its episode has ended and waits for this
+ * reset (t >= episode_length), auto_warmup carried over; before that, from tmpl.  Asynchronous on `stream`, except that
+ * a call with tmpl or streams uploads them through a staging buffer of its own and synchronises.  AIE_EINVAL for a reset_mode 0 config, a bad range
+ * or a missing array; AIE_ESTATE before aie_bind_buffers, or without tmpl and streams before anything was loaded. */
+typedef struct aie_reset_streams {
+    const uint32_t *mt_key;             /* [n, 624] numpy MT19937 key */
+    const int32_t *mt_pos;              /* [n] */
+    const int32_t *gauss_has;           /* [n] legacy Gaussian cache: required for lognormal skills and dynamic layouts */
+    const double *gauss_val;            /* [n] */
+    const double *split_skill;          /* [n, A] split_layout's rank -> build payment table (required there) */
+} aie_reset_streams;
+int aie_reset_envs(aie_env *env, const aie_host_state *tmpl, const aie_reset_streams *streams, int32_t env_lo, int32_t n,
+                   void *stream);
+
 /* Replaces: FoundationEnvWrapper.step_all_envs (env_wrapper.py:355-377) == BaseEnvironment.step
  * (base_env.py:929-1032) for every env: reads actions_*, advances `state`, writes obs/masks/reward/done. */
 int aie_step(aie_env *env, void *stream);
