@@ -4,9 +4,10 @@ import ctypes as C
 import numpy as np
 import os
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 MAX_COMPONENTS, MAX_BRACKETS, MAX_RATES = 8, 16, 64
 AIE_OK = 0
+OBS_F32, OBS_BF16 = 0, 1   # aie_config.obs_dtype
 
 COMPONENT_KIND = {"Build": 0, "ContinuousDoubleAuction": 1, "Gather": 2, "PeriodicBracketTax": 3,
                   "WealthRedistribution": 4, "SimpleLabor": 5}
@@ -49,6 +50,7 @@ class AieConfig(C.Structure):
         ("scenario_kind", C.c_int32), ("agent_reward_type", C.c_int32), ("labor_exponent", C.c_double), ("labor_cost", C.c_double),
         ("mz_partitions", C.c_int32 * 2), ("mz_zones", C.c_int32 * 3),
         ("labor_mask_first_step", C.c_int32), ("labor_skill_scale", C.c_double),
+        ("obs_dtype", C.c_int32),
     ]
 
 
@@ -215,6 +217,14 @@ EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field"
                     "aie_covid_sample_random_actions", "aie_covid_launch_count"]
 
 
+def obs_dtype_name(obs_dtype):
+    """"float32" or "bfloat16" for an obs_dtype kwarg: torch.float32 / torch.bfloat16, their names, or None (float32)."""
+    name = "float32" if obs_dtype is None else str(obs_dtype).replace("torch.", "")
+    if name not in ("float32", "bfloat16"):
+        raise ValueError("obs_dtype must be torch.float32 or torch.bfloat16, got %r" % (obs_dtype,))
+    return name
+
+
 def config_from_spec(spec, auto_reset=True):
     """spec: the flat numeric env description produced by foundation.spec.EnvSpec.to_dict()."""
     cfg = AieConfig()
@@ -260,6 +270,7 @@ def config_from_spec(spec, auto_reset=True):
     cfg.labor_cost = float(spec.get("labor_cost", 1.0))
     cfg.labor_mask_first_step = int(spec.get("labor_mask_first_step", 1))
     cfg.labor_skill_scale = float(spec.get("labor_skill_scale", 1.0))
+    cfg.obs_dtype = {"float32": OBS_F32, "bfloat16": OBS_BF16}[spec.get("obs_dtype", "float32")]
     cfg.dyn_layout = int(spec.get("dyn_layout", 0)) if cfg.reset_mode == 1 else 0
     if cfg.dyn_layout:
         cfg.dyn_checker = int(spec.get("dyn_checker", 0))

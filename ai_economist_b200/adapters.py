@@ -134,9 +134,11 @@ class WarpDriveStyleEnvWrapper:
 
     @staticmethod
     def _np_dtype(v):
+        """numpy dtype of a tensor's Box: bfloat16 observations (raw uint16 bits on numpy backends) get float32 spaces."""
         if isinstance(v, np.ndarray):
-            return v.dtype
-        return np.dtype(str(v.dtype).replace("torch.", ""))
+            return np.dtype(np.float32) if v.dtype == np.uint16 else v.dtype
+        name = str(v.dtype).replace("torch.", "")
+        return np.dtype(np.float32 if name == "bfloat16" else name)
 
     def tensor(self, name):
         """Device tensor registered under a WarpDrive-style name (cuda_data_manager.device_data(name))."""
@@ -241,8 +243,11 @@ class ReferenceApiEnv:
 
     # ---- output conversion -------------------------------------------------------------------------------
     def _np(self, v):
+        """numpy copy of an output tensor; bfloat16 observations as float32 (raw uint16 bits on numpy backends)."""
+        from .stepper import bf16_bits_to_float32
         st = self._env.stepper
-        return st.to_numpy(v) if not isinstance(v, np.ndarray) else v
+        a = st.to_numpy(v) if not isinstance(v, np.ndarray) else v
+        return bf16_bits_to_float32(a) if np.asarray(a).dtype == np.uint16 else a
 
     def _one(self, v):
         """The replica's slice of a batched value: arrays stay arrays, per-env scalars become Python floats."""

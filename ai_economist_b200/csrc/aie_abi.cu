@@ -9,6 +9,8 @@
 //   aie_finish_reset_kernel  one warp per env: tax trackers + utility metric_0 after a host reset upload.
 //   aie_reset_kernel       one warp per env: explicit reset on the device (aie_reset_envs), the auto-reset's re-draws.
 //   aie_metrics_kernel     one warp per env: env.metrics from the record in global memory, one row of a float64 table.
+// The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
+// aie_config::obs_dtype == AIE_OBS_BF16); the launchers pick one from the config, with the same launch shape.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -271,10 +273,10 @@ __device__ __forceinline__ void warp_step(const DevCfg &c, const DevBufs &b, int
 
 // ---------------------------------------------------------------------------------------------------------
 // One warp per env, up to 8 envs per CTA.  MINB = minimum resident CTAs per SM the register allocation targets
-// (occupancy vs. registers per thread); CS = the component kinds compiled in (step_comp_set).
-template <int MINB, bool EXT, int CS>
-__global__ void __launch_bounds__(256, MINB) aie_step_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
-                                                              const int emit_obs, const int env_lo) {
+// (occupancy vs. registers per thread); CS = the component kinds compiled in (step_comp_set); OT = the element type of
+// the float observations (aie_step_kernel: float, aie_step_bf16_kernel: bf16_t).
+template <bool EXT, int CS, typename OT>
+__device__ __forceinline__ void step_kernel_body(const DevCfg &c, const DevBufs &b, const int emit_obs, const int env_lo) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int wpb = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int env = env_lo + blockIdx.x * wpb + warp;   // the launch covers envs [env_lo, c.n_envs)
@@ -285,22 +287,41 @@ __global__ void __launch_bounds__(256, MINB) aie_step_kernel(const __grid_consta
     uint8_t *rec = warp_region(smem, wpb, warp, c);
     if (env < c.n_envs) warp_step<false, EXT, CS>(c, b, env, rec, bar, tab, lane);
     if (phase_sync) { __syncthreads(); if (env >= c.n_envs) return; }
-    if (emit_obs & 1) observe_env<EXT, CS>(c, rec, b.state + (size_t)env * c.rec_bytes, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<32, true>{lane});
+    if (emit_obs & 1) observe_env<EXT, CS, OT>(c, rec, b.state + (size_t)env * c.rec_bytes, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<32, true>{lane});
     else if (lane == 0) bulk_wait_read();
+}
+template <int MINB, bool EXT, int CS>
+__global__ void __launch_bounds__(256, MINB) aie_step_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
+                                                              const int emit_obs, const int env_lo) {
+    step_kernel_body<EXT, CS, float>(c, b, emit_obs, env_lo);
+}
+template <int MINB, bool EXT, int CS>
+__global__ void __launch_bounds__(256, MINB) aie_step_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
+                                                                   const int emit_obs, const int env_lo) {
+    step_kernel_body<EXT, CS, bf16_t>(c, b, emit_obs, env_lo);
 }
 
 // Large records: one CTA of four warps per env.  Warp 0 runs the (serial) dynamics; all four stream the observations.
-template <bool BIG, bool EXT = false>
-__global__ void __launch_bounds__(128, 4) aie_step_mw_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
-                                                             const int emit_obs, const int env_lo) {
+template <bool BIG, bool EXT, typename OT>
+__device__ __forceinline__ void step_mw_kernel_body(const DevCfg &c, const DevBufs &b, const int emit_obs, const int env_lo) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int env = env_lo + blockIdx.x;
     const uint16_t *tab = stage_tables(smem, 1, c, b);
     uint8_t *rec = warp_region(smem, 1, 0, c);
     if (threadIdx.x < 32) warp_step<BIG, EXT>(c, b, env, rec, (uint64_t *)smem, tab, threadIdx.x);
     __syncthreads();
-    if (emit_obs) observe_env<EXT>(c, rec, b.state + (size_t)env * c.rec_bytes, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<128, true>{(int)threadIdx.x});
+    if (emit_obs) observe_env<EXT, CS_ALL, OT>(c, rec, b.state + (size_t)env * c.rec_bytes, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<128, true>{(int)threadIdx.x});
     else if (threadIdx.x == 0) bulk_wait_read();
+}
+template <bool BIG, bool EXT = false>
+__global__ void __launch_bounds__(128, 4) aie_step_mw_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
+                                                             const int emit_obs, const int env_lo) {
+    step_mw_kernel_body<BIG, EXT, float>(c, b, emit_obs, env_lo);
+}
+template <bool BIG, bool EXT = false>
+__global__ void __launch_bounds__(128, 4) aie_step_mw_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
+                                                                  const int emit_obs, const int env_lo) {
+    step_mw_kernel_body<BIG, EXT, bf16_t>(c, b, emit_obs, env_lo);
 }
 
 __global__ void __launch_bounds__(256) aie_finish_reset_kernel(const __grid_constant__ DevCfg c, const DevBufs b,
@@ -410,8 +431,8 @@ __device__ __forceinline__ void load_obs_prefix(const DevCfg &c, uint8_t *rec, c
     if (!c.split) bulk_g2s(rec + c.off_price_hist, grec + c.off_price_hist, ph, bar);
     if (saez) bulk_g2s(rec + c.off_saez, grec + c.off_saez, saez, bar);
 }
-template <bool EXT>
-__global__ void __launch_bounds__(256) aie_observe_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+template <bool EXT, typename OT>
+__device__ __forceinline__ void observe_kernel_body(const DevCfg &c, const DevBufs &b, int lo, int n) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int wpb = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int i = blockIdx.x * wpb + warp;
@@ -424,10 +445,18 @@ __global__ void __launch_bounds__(256) aie_observe_kernel(const __grid_constant_
     if (lane == 0) load_obs_prefix(c, rec, grec, bar);
     __syncwarp();
     mbar_wait(bar, 0);
-    observe_env<EXT>(c, rec, grec, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<32, false>{lane});
+    observe_env<EXT, CS_ALL, OT>(c, rec, grec, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<32, false>{lane});
 }
 template <bool EXT>
-__global__ void __launch_bounds__(128, 4) aie_observe_mw_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+__global__ void __launch_bounds__(256) aie_observe_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+    observe_kernel_body<EXT, float>(c, b, lo, n);
+}
+template <bool EXT>
+__global__ void __launch_bounds__(256) aie_observe_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+    observe_kernel_body<EXT, bf16_t>(c, b, lo, n);
+}
+template <bool EXT, typename OT>
+__device__ __forceinline__ void observe_mw_kernel_body(const DevCfg &c, const DevBufs &b, int lo, int n) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int env = lo + blockIdx.x;
     const uint16_t *tab = stage_tables(smem, 1, c, b);
@@ -437,7 +466,15 @@ __global__ void __launch_bounds__(128, 4) aie_observe_mw_kernel(const __grid_con
     if (threadIdx.x == 0) load_obs_prefix(c, rec, grec, bar);
     __syncthreads();
     mbar_wait(bar, 0);
-    observe_env<EXT>(c, rec, grec, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<128, false>{(int)threadIdx.x});
+    observe_env<EXT, CS_ALL, OT>(c, rec, grec, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<128, false>{(int)threadIdx.x});
+}
+template <bool EXT>
+__global__ void __launch_bounds__(128, 4) aie_observe_mw_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+    observe_mw_kernel_body<EXT, float>(c, b, lo, n);
+}
+template <bool EXT>
+__global__ void __launch_bounds__(128, 4) aie_observe_mw_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+    observe_mw_kernel_body<EXT, bf16_t>(c, b, lo, n);
 }
 
 // Episode metrics (aie_metrics.cuh): one warp per env, eight per CTA, reads the env's record (current or end-of-episode
@@ -453,20 +490,29 @@ __global__ void __launch_bounds__(256) aie_metrics_kernel(const __grid_constant_
 
 // per_unit == 0: one warp per env (fastest for few agents: c2 15.2 us vs 17.5 us);  per_unit == 1: one warp per
 // (env, agent | planner bracket) - many agents x subspaces make the per-env chain long (c5: 64 agents x 6 subspaces).
-template <bool EXT>
-__global__ void __launch_bounds__(256) aie_sample_kernel(const __grid_constant__ DevCfg c, const DevBufs b, uint64_t seed,
-                                                         int per_unit) {
+template <bool EXT, typename MT>
+__device__ __forceinline__ void sample_kernel_body(const DevCfg &c, const DevBufs &b, uint64_t seed, int per_unit) {
     const long long wid = (long long)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
     const int lane = threadIdx.x & 31;
     const int units = per_unit ? c.A + (c.planner_acts ? c.B : 0) : 1;
     const int env = (int)(wid / units), u = (int)(wid - (long long)env * units);
     if (env >= c.n_envs) return;
-    const float *am = b.a_mask + (size_t)env * c.A * c.Na, *pm = b.p_mask + (size_t)env * c.Np;
+    const MT *am = (const MT *)b.a_mask + (size_t)env * c.A * c.Na, *pm = (const MT *)b.p_mask + (size_t)env * c.Np;
     int32_t *aa = const_cast<int32_t *>(b.act_a) + (size_t)env * c.A * c.n_act_a;
     int32_t *ap = c.n_act_p ? const_cast<int32_t *>(b.act_p) + (size_t)env * c.n_act_p : nullptr;
     const uint64_t key = mix64(seed ^ mix64((uint64_t)env));
     if (per_unit) sample_actions_unit<EXT>(c, am, pm, aa, ap, key, u, lane);
     else sample_actions_env<EXT>(c, am, pm, aa, ap, key, lane);
+}
+template <bool EXT>
+__global__ void __launch_bounds__(256) aie_sample_kernel(const __grid_constant__ DevCfg c, const DevBufs b, uint64_t seed,
+                                                         int per_unit) {
+    sample_kernel_body<EXT, float>(c, b, seed, per_unit);
+}
+template <bool EXT>   // reads bfloat16 masks
+__global__ void __launch_bounds__(256) aie_sample_bf16_kernel(const __grid_constant__ DevCfg c, const DevBufs b, uint64_t seed,
+                                                              int per_unit) {
+    sample_kernel_body<EXT, bf16_t>(c, b, seed, per_unit);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -551,6 +597,14 @@ int init(aie_env *env) {
     AIE_OPT_IN(aie_reset_kernel<false>); AIE_OPT_IN(aie_reset_kernel<true>);
     AIE_OPT_IN(aie_observe_kernel<false>); AIE_OPT_IN(aie_observe_kernel<true>);
     AIE_OPT_IN(aie_observe_mw_kernel<false>); AIE_OPT_IN(aie_observe_mw_kernel<true>);
+    AIE_OPT_IN((aie_step_bf16_kernel<3, false, CS_GTB>)); AIE_OPT_IN((aie_step_bf16_kernel<4, false, CS_GTB>));
+    AIE_OPT_IN((aie_step_bf16_kernel<3, false, CS_GTB_TAX>)); AIE_OPT_IN((aie_step_bf16_kernel<4, false, CS_GTB_TAX>));
+    AIE_OPT_IN((aie_step_bf16_kernel<3, false, CS_ALL>)); AIE_OPT_IN((aie_step_bf16_kernel<4, false, CS_ALL>));
+    AIE_OPT_IN((aie_step_bf16_kernel<3, true, CS_ALL>)); AIE_OPT_IN((aie_step_bf16_kernel<4, true, CS_ALL>));
+    AIE_OPT_IN((aie_step_mw_bf16_kernel<false, false>)); AIE_OPT_IN((aie_step_mw_bf16_kernel<false, true>));
+    AIE_OPT_IN((aie_step_mw_bf16_kernel<true, false>)); AIE_OPT_IN((aie_step_mw_bf16_kernel<true, true>));
+    AIE_OPT_IN(aie_observe_bf16_kernel<false>); AIE_OPT_IN(aie_observe_bf16_kernel<true>);
+    AIE_OPT_IN(aie_observe_mw_bf16_kernel<false>); AIE_OPT_IN(aie_observe_mw_bf16_kernel<true>);
 #undef AIE_OPT_IN
     {
         AIE_CUDA(cudaMalloc((void **)&env->be.tab_dev, sizeof(Tables)), "cudaMalloc tables");
@@ -708,21 +762,31 @@ int launch_step_range(aie_env *env, int emit_obs, int lo, int hi, void *stream) 
     const DevCfg &cfg = *cp;
     if (env->cfg.mw > 1) {   // large records: one CTA of four warps per env
         const dim3 grid(n), block(32 * env->cfg.mw);
-        if (env->cfg.ext) {
-            if (env->cfg.split) aie_step_mw_kernel<true, true><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
-            else aie_step_mw_kernel<false, true><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
-        } else if (env->cfg.split) aie_step_mw_kernel<true, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
-        else aie_step_mw_kernel<false, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);
+#define AIE_STEP_MW(K) do {                                                                               \
+        if (env->cfg.ext) {                                                                               \
+            if (env->cfg.split) K<true, true><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);     \
+            else K<false, true><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);                   \
+        } else if (env->cfg.split) K<true, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo); \
+        else K<false, false><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo);                      \
+    } while (0)
+        if (env->cfg.obs_bf16) AIE_STEP_MW(aie_step_mw_bf16_kernel);
+        else AIE_STEP_MW(aie_step_mw_kernel);
+#undef AIE_STEP_MW
     } else {
         const dim3 grid((n + wpb - 1) / wpb), block(wpb * 32);
         const bool m4 = env->be.step_minb == 4;
-#define AIE_STEP(EXT, CS) (m4 ? aie_step_kernel<4, EXT, CS><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo) \
-                              : aie_step_kernel<3, EXT, CS><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo))
+#define AIE_STEP(K, EXT, CS) (m4 ? K<4, EXT, CS><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo) \
+                                 : K<3, EXT, CS><<<grid, block, sm, st>>>(cfg, env->bufs, emit_obs, lo))
         // EXT: rarely used options compiled in (single-action planner, regen halfwidth), with every component kind
-        if (env->cfg.ext) AIE_STEP(true, CS_ALL);
-        else if (env->be.step_cs == CS_GTB) AIE_STEP(false, CS_GTB);
-        else if (env->be.step_cs == CS_GTB_TAX) AIE_STEP(false, CS_GTB_TAX);
-        else AIE_STEP(false, CS_ALL);
+#define AIE_STEP_CS(K) do {                                                        \
+        if (env->cfg.ext) AIE_STEP(K, true, CS_ALL);                               \
+        else if (env->be.step_cs == CS_GTB) AIE_STEP(K, false, CS_GTB);            \
+        else if (env->be.step_cs == CS_GTB_TAX) AIE_STEP(K, false, CS_GTB_TAX);    \
+        else AIE_STEP(K, false, CS_ALL);                                           \
+    } while (0)
+        if (env->cfg.obs_bf16) AIE_STEP_CS(aie_step_bf16_kernel);
+        else AIE_STEP_CS(aie_step_kernel);
+#undef AIE_STEP_CS
 #undef AIE_STEP
     }
     AIE_CUDA(cudaGetLastError(), "aie_step_kernel launch");
@@ -732,11 +796,16 @@ int launch_step_range(aie_env *env, int emit_obs, int lo, int hi, void *stream) 
 int launch_observe(aie_env *env, int lo, int n, void *stream) {
     const int wpb = env->be.step_wpb;
     cudaStream_t st = (cudaStream_t)stream;
-    if (env->cfg.mw > 1) {
-        if (env->cfg.ext) aie_observe_mw_kernel<true><<<n, 32 * env->cfg.mw, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);
-        else aie_observe_mw_kernel<false><<<n, 32 * env->cfg.mw, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);
-    } else if (env->cfg.ext) aie_observe_kernel<true><<<(n + wpb - 1) / wpb, wpb * 32, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);
-    else aie_observe_kernel<false><<<(n + wpb - 1) / wpb, wpb * 32, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);
+#define AIE_OBSERVE(K, KMW) do {                                                                                                       \
+    if (env->cfg.mw > 1) {                                                                                                             \
+        if (env->cfg.ext) KMW<true><<<n, 32 * env->cfg.mw, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);                       \
+        else KMW<false><<<n, 32 * env->cfg.mw, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);                                   \
+    } else if (env->cfg.ext) K<true><<<(n + wpb - 1) / wpb, wpb * 32, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);            \
+    else K<false><<<(n + wpb - 1) / wpb, wpb * 32, env->be.obs_smem, st>>>(env->cfg, env->bufs, lo, n);                               \
+} while (0)
+    if (env->cfg.obs_bf16) AIE_OBSERVE(aie_observe_bf16_kernel, aie_observe_mw_bf16_kernel);
+    else AIE_OBSERVE(aie_observe_kernel, aie_observe_mw_kernel);
+#undef AIE_OBSERVE
     AIE_CUDA(cudaGetLastError(), "aie_observe_kernel launch");
     env->launches++;
     return AIE_OK;
@@ -758,8 +827,13 @@ int launch_sample(aie_env *env, uint64_t seed, void *stream) {
     const int per_unit = (env->cfg.A * (env->cfg.multi_action ? env->cfg.n_sub : 1) >= 64) ? 1 : 0;
     const long long warps = (long long)env->n_envs * (per_unit ? units : 1);
     const uint64_t sd = host_mix64(seed) ^ host_mix64(++env->sample_calls);
-    if (env->cfg.ext) aie_sample_kernel<true><<<(unsigned)((warps + 7) / 8), 256, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, sd, per_unit);
-    else aie_sample_kernel<false><<<(unsigned)((warps + 7) / 8), 256, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, sd, per_unit);
+    const unsigned grid = (unsigned)((warps + 7) / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (env->cfg.obs_bf16) {
+        if (env->cfg.ext) aie_sample_bf16_kernel<true><<<grid, 256, 0, st>>>(env->cfg, env->bufs, sd, per_unit);
+        else aie_sample_bf16_kernel<false><<<grid, 256, 0, st>>>(env->cfg, env->bufs, sd, per_unit);
+    } else if (env->cfg.ext) aie_sample_kernel<true><<<grid, 256, 0, st>>>(env->cfg, env->bufs, sd, per_unit);
+    else aie_sample_kernel<false><<<grid, 256, 0, st>>>(env->cfg, env->bufs, sd, per_unit);
     AIE_CUDA(cudaGetLastError(), "aie_sample_kernel launch");
     env->launches++;
     return AIE_OK;

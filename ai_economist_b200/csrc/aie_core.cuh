@@ -25,8 +25,12 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "aie_layout.h"
+#if defined(__CUDACC__) && !defined(AIE_EMU)
+#include <cuda_bf16.h>
+#endif
 
 #if defined(__CUDACC__) && !defined(AIE_EMU)
 #define AIE_DEV __device__ __forceinline__
@@ -1525,7 +1529,11 @@ AIE_DEV uint64_t mix64(uint64_t x) {  // splitmix64 finaliser
 }
 // Uniform choice among the set entries of mask[0..n) by one warp: ballots count the open entries, a hashed
 // rank picks one, and the lane holding it is found with popcounts.  Returns the same value on every lane.
-AIE_DEV int sample_segment_warp(const float *mask, int n, uint64_t key, int lane) {
+// (masks are 0 / 1: any non-zero element is open; MT: float or bf16_t)
+AIE_DEV bool mask_open(float v) { return v != 0.0f; }
+AIE_DEV bool mask_open(bf16_t v) { return (v.bits & 0x7FFFu) != 0u; }
+template <typename MT>
+AIE_DEV int sample_segment_warp(const MT *mask, int n, uint64_t key, int lane) {
 #if AIE_ON_DEVICE
     // one pass: the segment (at most MAX_MASK = 160 entries) becomes five ballot words held in registers
     uint32_t w[5];
@@ -1533,7 +1541,7 @@ AIE_DEV int sample_segment_warp(const float *mask, int n, uint64_t key, int lane
 #pragma unroll
     for (int ch = 0; ch < 5; ch++) {
         const int j = ch * NL + lane;
-        w[ch] = wballot(j < n && mask[j] != 0.0f);
+        w[ch] = wballot(j < n && mask_open(mask[j]));
         total += __popc(w[ch]);
     }
     if (total == 0) return 0;
@@ -1549,13 +1557,13 @@ AIE_DEV int sample_segment_warp(const float *mask, int n, uint64_t key, int lane
     int total = 0;
     for (int base = 0; base < n; base += NL) {
         const int j = base + lane;
-        total += __popc_u32(wballot(j < n && mask[j] != 0.0f));
+        total += __popc_u32(wballot(j < n && mask_open(mask[j])));
     }
     if (total == 0) return 0;
     int r = (int)((uint32_t)(mix64(key) >> 32) % (uint32_t)total);
     for (int base = 0; base < n; base += NL) {
         const int j = base + lane;
-        const uint32_t m = wballot(j < n && mask[j] != 0.0f);
+        const uint32_t m = wballot(j < n && mask_open(mask[j]));
         const int cnt = __popc_u32(m);
         if (r < cnt) {
             uint32_t mm = m;
@@ -1570,12 +1578,12 @@ AIE_DEV int sample_segment_warp(const float *mask, int n, uint64_t key, int lane
 
 // One unit of an env's random policy: unit u < A = agent u (one draw per subspace), unit A + b = planner bracket b.
 // Units are independent, so the kernel gives each its own warp.
-template <bool EXT = false>
-AIE_DEV void sample_actions_unit(const DevCfg &c, const float *a_mask, const float *p_mask, int32_t *act_a,
+template <bool EXT = false, typename MT = float>
+AIE_DEV void sample_actions_unit(const DevCfg &c, const MT *a_mask, const MT *p_mask, int32_t *act_a,
                                  int32_t *act_p, uint64_t key, int u, int lane) {
     if (u < c.A) {
         const int a = u;
-        const float *m = a_mask + (size_t)a * c.Na;
+        const MT *m = a_mask + (size_t)a * c.Na;
         if (!c.multi_action) {
             const int v = sample_segment_warp(m, c.Na, key + 0x100 * a, lane);
             if (lane == 0) act_a[a] = v;
@@ -1599,11 +1607,11 @@ AIE_DEV void sample_actions_unit(const DevCfg &c, const float *a_mask, const flo
     }
 }
 // One env: every agent (and planner bracket) draws one uniformly random unmasked action per subspace.
-template <bool EXT = false>
-AIE_DEV void sample_actions_env(const DevCfg &c, const float *a_mask, const float *p_mask, int32_t *act_a,
+template <bool EXT = false, typename MT = float>
+AIE_DEV void sample_actions_env(const DevCfg &c, const MT *a_mask, const MT *p_mask, int32_t *act_a,
                                 int32_t *act_p, uint64_t key, int lane) {
     const int units = c.A + (c.planner_acts ? c.B : 0);
-    for (int u = 0; u < units; u++) sample_actions_unit<EXT>(c, a_mask, p_mask, act_a, act_p, key, u, lane);
+    for (int u = 0; u < units; u++) sample_actions_unit<EXT, MT>(c, a_mask, p_mask, act_a, act_p, key, u, lane);
 }
 
 }  // namespace aie

@@ -54,6 +54,7 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
     memset(&tb, 0, sizeof(tb));
     auto bad = [&](const char *m) { err = m; return AIE_EINVAL; };
     if (u.abi_version != AIE_ABI_VERSION) return bad("abi_version mismatch");
+    if (u.obs_dtype != AIE_OBS_F32 && u.obs_dtype != AIE_OBS_BF16) return bad("obs_dtype must be AIE_OBS_F32 or AIE_OBS_BF16");
     if (n_envs < 1) return bad("n_envs must be >= 1");
     if (u.n_agents < 2 || u.n_agents > AIE_MAX_AGENTS) return bad("n_agents must be in [2, 64]");
     if (u.height < 1 || u.width < 1 || u.height > 256 || u.width > 256) return bad("world size must be within 256x256");
@@ -150,6 +151,7 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
             return bad("fixed_four start cell outside the world");
     }
     c.n_envs = n_envs;
+    c.obs_bf16 = u.obs_dtype == AIE_OBS_BF16 ? 1 : 0;
 
     // action subspaces in component-list order (base_agent.py:124-169)
     int lo = 1, n_single = 0;
@@ -307,6 +309,10 @@ inline int build_devcfg(const aie_config &u, int n_envs, DevCfg &c, Tables &tb, 
         c.tab_lut = (c.tab_seg + n_seg + 7) & ~7;   // 16-byte aligned (u16 words)
         float *lut = (float *)(tb.w + c.tab_lut);   // nibble -> four floats (bit k of the nibble -> element k)
         for (int k = 0; k < 16; k++) for (int j = 0; j < 4; j++) lut[4 * k + j] = (float)((k >> j) & 1);
+        if (c.obs_bf16) {   // nibble -> four bfloat16 (8 bytes), in the same slot
+            uint16_t *lut16 = tb.w + c.tab_lut;
+            for (int k = 0; k < 16; k++) for (int j = 0; j < 4; j++) lut16[4 * k + j] = (uint16_t)(((k >> j) & 1) ? 0x3F80u : 0u);
+        }
         c.tab_n = c.tab_lut + 128;
         // compacted transfer: every entry of the agents' flat program gets its index inside its class
         c.tab_cslot = c.tab_n;
@@ -548,8 +554,9 @@ inline void fill_dims(const DevCfg &c, aie_dims &d) {
     d.state_bytes = c.rec_bytes;
     d.n_stats = c.n_stats; d.stats_trade = c.st_trade; d.stats_tax = c.st_tax;
     d.agent_map_elems = c.a_map_elems; d.agent_idx_elems = c.a_idx_elems;
-    long long obs = (long long)c.A * (c.a_map_elems * 4 + c.a_idx_elems * 2 + c.Fa * 4 + c.Na * 4) + c.Fp * 4 + c.A * c.Fpa * 4 +
-                    c.Np * 4 + 4 + (c.planner_spatial ? (c.M * c.HW * 4 + 2 * c.HW * 2) : 0);
+    const int fb = c.obs_bf16 ? 2 : 4;   // bytes per element of the float tensors
+    long long obs = (long long)c.A * (c.a_map_elems * fb + c.a_idx_elems * 2 + c.Fa * fb + c.Na * fb) + c.Fp * fb + c.A * c.Fpa * fb +
+                    c.Np * fb + fb + (c.planner_spatial ? (c.M * c.HW * fb + 2 * c.HW * 2) : 0);
     long long io = 8 * (c.A + 1) + 4 + 4 * (c.A * c.n_act_a + c.n_act_p);
     d.algorithmic_bytes_per_env_step = (int32_t)(obs + io + 2LL * c.rec_bytes);
 }

@@ -169,6 +169,8 @@ struct DevCfg {
     int32_t dyn_layout, dyn_checker;
     double dyn_cov[2], dyn_clump[2];   // [Wood, Stone]
     int32_t mz_rows, mz_cols, mz_psr, mz_psc, mz_zones[3];   // MultiZone: partitions, partition size in cells, zones per type
+    // aie_config::obs_dtype == AIE_OBS_BF16: the float observation / mask tensors are bfloat16 (the *_bf16 kernels)
+    int32_t obs_bf16;
 };
 
 // raw device pointers (mirrors aie_buffers)
@@ -201,7 +203,8 @@ struct ResetSrc {
     int32_t counters_from_record; // 1: completions / auto_warmup come from the current record, 0: from tmpl
 };
 // compact program table: [agent flat (Fa) | planner flat (Fp) | p<i> flat (Fpa) | agent mask (Na)], offsets in DevCfg
-// then: histogram offsets u16 [4P <= 128], mask segments u16 [<= 64], nibble -> float4 table (64 floats = 128 u16)
+// then: histogram offsets u16 [4P <= 128], mask segments u16 [<= 64], nibble -> float4 table (64 floats = 128 u16; with
+// bfloat16 output the first 64 u16 hold the nibble -> four-bf16 table instead)
 constexpr int TAB_WORDS = 2 * MAX_FLAT + 16 + MAX_MASK + 128 + 64 + 128 + 16 + MAX_FLAT;
 struct Tables { uint16_t w[TAB_WORDS]; };
 

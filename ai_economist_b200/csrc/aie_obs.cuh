@@ -20,9 +20,38 @@
 //   3. stream: every 16-byte group of the run is lut[nibble] - one shared-memory word, a shift, a 16-entry float4 table
 //      lookup and one 16-byte store per thread per iteration, front to back in address order.
 // Index planes stream as bytes -> int16, flat vectors / masks as table-driven gathers, each as ONE run per tensor slice.
+//
+// Output element type OT.  The float tensors (maps, flat vectors, masks, time) are float32 (OT = float), or bfloat16
+// (OT = bf16_t, aie_config::obs_dtype == AIE_OBS_BF16): every value is computed in float32 as for float32 output and
+// rounded to nearest even on the way out, 8 elements per 16-byte group instead of 4.
 #pragma once
 
 namespace aie {
+
+// ---- bfloat16 output ---------------------------------------------------------------------------------------------
+struct bf16_t { uint16_t bits; };   // bfloat16 storage
+// round-to-nearest-even bfloat16 bits of v (what torch's float32 -> bfloat16 conversion gives; NaN -> a quiet NaN)
+AIE_DEV uint32_t bf16_rn(float v) {
+#if AIE_ON_DEVICE
+    return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+#else
+    uint32_t u;
+    memcpy(&u, &v, 4);
+    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return 0x7FC0u;
+    return (u + 0x7FFFu + ((u >> 16) & 1u)) >> 16;
+#endif
+}
+AIE_DEV uint32_t bf16x2_rn(float lo, float hi) {   // two values, lo in the low half (the lower address)
+#if AIE_ON_DEVICE
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+#else
+    return bf16_rn(lo) | (bf16_rn(hi) << 16);
+#endif
+}
+AIE_DEV void put_out(float *p, float v) { *p = v; }
+AIE_DEV void put_out(bf16_t *p, float v) { p->bits = (uint16_t)bf16_rn(v); }
 
 // ---- executors ---------------------------------------------------------------------------------------------------
 // host: runs a phase for every thread index of the group, one after the other (phases only read earlier phases' data)
@@ -75,6 +104,11 @@ AIE_DEV void store_edges(T *dst, const RunSplit &r, int n, int tid, int NT, F va
     const int ne = r.head + (n - r.tail0);
     for (int j = tid; j < ne; j += NT) { const int i = j < r.head ? j : r.tail0 + (j - r.head); dst[i] = (T)value_at(i); }
 }
+template <typename F>
+AIE_DEV void store_edges(bf16_t *dst, const RunSplit &r, int n, int tid, int NT, F value_at) {   // (<= 7 + 7 elements)
+    const int ne = r.head + (n - r.tail0);
+    for (int j = tid; j < ne; j += NT) { const int i = j < r.head ? j : r.tail0 + (j - r.head); put_out(dst + i, value_at(i)); }
+}
 // rows x n matrix, contiguous: dst[row * n + i] = value_at(row, i), written as ONE run (n_magic = floor(2^32 / n) + 1; not
 // read when rows == 1).  Thread tid owns the 16-byte groups tid, tid + NT, ... of the destination: it computes the group's
 // values in registers, one after the other through a single value_at site (the small code matters more than the three
@@ -110,6 +144,51 @@ AIE_DEV void store_rows_f32(float *dst, int rows, int n, uint32_t n_magic, int t
             if (x0 + 3 < total) q[3] = v3;
         }
     }
+}
+// The same for bfloat16 output: eight values per 16-byte group, rounded in pairs into four words (one value_at site).
+template <typename F>
+AIE_DEV void store_rows_bf16(bf16_t *dst, int rows, int n, uint32_t n_magic, int tid, int NT, F value_at) {
+    const int total = rows * n;
+    const int a = (int)(((uintptr_t)dst >> 1) & 7);   // elements in front of the run inside its first 16-byte group
+    const int ng = (a + total + 7) >> 3;
+#if AIE_ON_DEVICE
+    AIE_UNROLL(1)
+#endif
+    for (int k = tid; k < ng; k += NT) {
+        const int x0 = 8 * k - a;
+        const int xs = x0 > 0 ? x0 : 0;
+        int row = rows > 1 ? (int)div_magic((uint32_t)xs, n_magic) : 0, i = xs - row * n;
+        uint32_t w0 = 0u, w1 = 0u, w2 = 0u, w3 = 0u;
+        float lo = 0.0f;
+#if AIE_ON_DEVICE
+        AIE_UNROLL(1)
+#endif
+        for (int x = x0; x < x0 + 8; x++) {
+            float v = 0.0f;
+            if (x >= 0 && x < total) { v = value_at(row, i); if (++i == n) { i = 0; row++; } }
+            if (((x - x0) & 1) == 0) { lo = v; } else { w0 = w1; w1 = w2; w2 = w3; w3 = bf16x2_rn(lo, v); }
+        }
+        bf16_t *q = dst + x0;
+        if (x0 >= 0 && x0 + 8 <= total) {
+            store8(reinterpret_cast<int16_t *>(q), w0, w1, w2, w3);
+        } else {
+#if AIE_ON_DEVICE
+            AIE_UNROLL(1)
+#endif
+            for (int j = 0; j < 8; j++) {   // element j is the low half of w0 after j shifts
+                if (x0 + j >= 0 && x0 + j < total) q[j].bits = (uint16_t)w0;
+                w0 = fshr(w0, w1, 16); w1 = fshr(w1, w2, 16); w2 = fshr(w2, w3, 16); w3 >>= 16;
+            }
+        }
+    }
+}
+template <typename F>
+AIE_DEV void store_rows(float *dst, int rows, int n, uint32_t n_magic, int tid, int NT, F value_at) {
+    store_rows_f32(dst, rows, n, n_magic, tid, NT, value_at);
+}
+template <typename F>
+AIE_DEV void store_rows(bf16_t *dst, int rows, int n, uint32_t n_magic, int tid, int NT, F value_at) {
+    store_rows_bf16(dst, rows, n, n_magic, tid, NT, value_at);
 }
 // dst[i] = code(bytes[i]) widened to int16, code = identity (OWNER == false) or the house-owner encoding of an
 // int8 owner byte (-1 -> 0, a -> a + 2; layout_from_file.py:438-440) applied four bytes at a time.
@@ -244,11 +323,58 @@ AIE_DEV void stream_bits_f32(float *dst, int total, const uint32_t *bits, const 
     }
 #endif
 }
+// bfloat16 output: group g of the run is byte g of the bit string, two lut entries of four bf16 (8 bytes) each;
+// lut8[2 * k], lut8[2 * k + 1] = the words of nibble k (bit j of the nibble -> element j).  Thread tid owns groups tid,
+// tid + NT, ...: its byte index advances by NT per group; four groups per iteration.
+AIE_DEV void stream_bits_bf16(bf16_t *dst, int total, const uint32_t *bits, const uint32_t *lut8, const uint8_t *planes,
+                              int stride, int n, uint32_t n_magic, int tid, int NT) {
+    const RunSplit r = run_split(dst, total, 1);
+    store_edges(dst, r, total, tid, NT, [&](int x) { return plane_value(planes, stride, n, n_magic, x); });
+    const uint8_t *b8 = reinterpret_cast<const uint8_t *>(bits) + tid;
+    int g = tid;
+#if AIE_ON_DEVICE
+    const uint2 *lut2 = reinterpret_cast<const uint2 *>(lut8);
+    uint4 *q4 = reinterpret_cast<uint4 *>(dst + r.head) + tid;
+    auto group = [&](uint32_t v) {
+        const uint2 lo = lut2[v & 15u], hi = lut2[v >> 4];
+        return make_uint4(lo.x, lo.y, hi.x, hi.y);
+    };
+    AIE_UNROLL(1)
+    for (; g + 3 * NT < r.nq; g += 4 * NT) {
+        const uint32_t v0 = b8[0], v1 = b8[NT], v2 = b8[2 * NT], v3 = b8[3 * NT];
+        __stcs(q4, group(v0)); __stcs(q4 + NT, group(v1));
+        __stcs(q4 + 2 * NT, group(v2)); __stcs(q4 + 3 * NT, group(v3));
+        b8 += 4 * NT; q4 += 4 * NT;
+    }
+    AIE_UNROLL(1)
+    for (; g < r.nq; g += NT) { __stcs(q4, group(b8[0])); b8 += NT; q4 += NT; }
+#else
+    int16_t *q = reinterpret_cast<int16_t *>(dst + r.head) + 8 * tid;
+    for (; g < r.nq; g += NT) {
+        const uint32_t lo = b8[0] & 15u, hi = b8[0] >> 4;
+        store8(q, lut8[2 * lo], lut8[2 * lo + 1], lut8[2 * hi], lut8[2 * hi + 1]);
+        b8 += NT; q += 8 * NT;
+    }
+#endif
+}
+AIE_DEV void stream_bits(float *dst, int total, const uint32_t *bits, const uint16_t *lut, const uint8_t *planes, int stride,
+                         int n, uint32_t n_magic, int tid, int NT) {
+    stream_bits_f32(dst, total, bits, reinterpret_cast<const float *>(lut), planes, stride, n, n_magic, tid, NT);
+}
+AIE_DEV void stream_bits(bf16_t *dst, int total, const uint32_t *bits, const uint16_t *lut, const uint8_t *planes, int stride,
+                         int n, uint32_t n_magic, int tid, int NT) {
+    stream_bits_bf16(dst, total, bits, reinterpret_cast<const uint32_t *>(lut), planes, stride, n, n_magic, tid, NT);
+}
 // how many words of bit string a run at `dst` needs (whole 16-byte groups only)
 AIE_DEV int bits_words_for(const float *dst, int total, int *head) {
     const RunSplit r = run_split(dst, total, 2);
     *head = r.head;
     return (4 * r.nq + 31) >> 5;
+}
+AIE_DEV int bits_words_for(const bf16_t *dst, int total, int *head) {
+    const RunSplit r = run_split(dst, total, 1);
+    *head = r.head;
+    return (8 * r.nq + 31) >> 5;
 }
 
 // ---- staging -------------------------------------------------------------------------------------------------------
@@ -280,19 +406,19 @@ AIE_DEV ObsScratch obs_scratch_view(uint8_t *base, const int32_t *ob) {
 }
 
 // Output slices of one env, computed where they are used (keeping ten 64-bit pointers live through the pass would
-// spill under the register budget).
+// spill under the register budget).  OT: the element type of the float tensors (their buffers hold OT when bfloat16).
 struct ObsOut {
     const DevBufs *b; const DevCfg *c; size_t env;
-    AIE_DEV_MEMBER float *a_map() const { return b->a_map + env * c->A * c->a_map_elems; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *a_map() const { return (OT *)b->a_map + env * c->A * c->a_map_elems; }
     AIE_DEV_MEMBER int16_t *a_idx() const { return b->a_idx + env * c->A * c->a_idx_elems; }
-    AIE_DEV_MEMBER float *a_flat() const { return b->a_flat + env * c->A * c->Fa; }
-    AIE_DEV_MEMBER float *a_mask() const { return b->a_mask + env * c->A * c->Na; }
-    AIE_DEV_MEMBER float *p_map() const { return b->p_map + env * c->M * c->HW; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *a_flat() const { return (OT *)b->a_flat + env * c->A * c->Fa; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *a_mask() const { return (OT *)b->a_mask + env * c->A * c->Na; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *p_map() const { return (OT *)b->p_map + env * c->M * c->HW; }
     AIE_DEV_MEMBER int16_t *p_idx() const { return b->p_idx + env * 2 * c->HW; }
-    AIE_DEV_MEMBER float *p_flat() const { return b->p_flat + env * c->Fp; }
-    AIE_DEV_MEMBER float *p_agents() const { return b->p_agents + env * c->A * c->Fpa; }
-    AIE_DEV_MEMBER float *p_mask() const { return b->p_mask + env * c->Np; }
-    AIE_DEV_MEMBER float *time_obs() const { return b->time_obs + env; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *p_flat() const { return (OT *)b->p_flat + env * c->Fp; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *p_agents() const { return (OT *)b->p_agents + env * c->A * c->Fpa; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *p_mask() const { return (OT *)b->p_mask + env * c->Np; }
+    template <typename OT = float> AIE_DEV_MEMBER OT *time_obs() const { return (OT *)b->time_obs + env; }
 };
 
 // One element of a "flat" vector (program entry -> value).  FK_SHARED: the per-env shared float staging; FK_AGENT: agent
@@ -331,16 +457,21 @@ AIE_DEV int policy_pick(const uint16_t *seg, int s0, int s1, const uint8_t *lim,
     return 0;
 }
 
-// CS: the component kinds compiled in (see step_env)
-template <bool EXT, int CS = CS_ALL, class Exec>
+// CS: the component kinds compiled in (see step_env); OT: the output element type of the float tensors (float, bf16_t).
+template <bool EXT, int CS = CS_ALL, typename OT = float, class Exec>
 AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *stage_base, const int32_t *ob, const ObsOut &o,
                          const uint16_t *tab, const Exec &ex) {
+#if !AIE_ON_DEVICE
+    // host build of the device source: one entry for both element types, picked from the config as the CUDA launchers
+    // pick the bfloat16 kernels
+    if (sizeof(OT) == 4 && c.obs_bf16) { observe_env<EXT, CS, bf16_t>(c, rec, grec, stage_base, ob, o, tab, ex); return; }
+#endif
     const Env e = env_view(rec, grec, c);
     const ObsScratch s = obs_scratch_view(stage_base, ob);
     const int NT = ex.nt();
     const int A = c.A, H = c.H, W = c.W, HW = c.HW, P = c.P, M = c.M, win = c.win, w = c.w, ww = win * win;
     const double inv_scale = c.obs_scaling ? 0.01 : 1.0;
-    const float *lut = reinterpret_cast<const float *>(tab + c.tab_lut);
+    const uint16_t *lut = tab + c.tab_lut;   // nibble -> 4 elements of OT (float4 / four bf16)
     const uint16_t *hoff = tab + c.tab_hoff;
 
     // ---- phase A: stage every scalar the flat vectors / masks need (float, final values) -------------
@@ -389,7 +520,7 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
                 s.sc_a[a * AS_COUNT + AS_TAX_LAST_MARG] = (float)e.last_marg[a];
             }
         }
-        if (tid == 0) { s.shf[SH_ZERO] = 0.0f; s.shf[SH_TIME] = (float)time_v; o.time_obs()[0] = (float)time_v; }
+        if (tid == 0) { s.shf[SH_ZERO] = 0.0f; s.shf[SH_TIME] = (float)time_v; put_out(o.time_obs<OT>(), (float)time_v); }
     });
     ex([&](int tid) {
         for (int a = tid; a < A; a += NT) {
@@ -474,29 +605,29 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
 
     // ---- phase B: the flat vectors and masks (base_env.py:562-612, base_agent.py:440-460), the policy ----------------
     // Every flat / mask tensor is ONE run written straight from the staged scalars / limits: the four values of a 16-byte
-    // group are computed in registers and stored together (store_rows_f32).
+    // group are computed in registers and stored together (store_rows).
     ex([&](int tid) {
         const float *shf = s.shf;
         const uint8_t *hist = e.bid_hist;
         const int sh_full = c.sh_full;
         {   // the planner's flat vector
             const uint16_t *tp = tab + c.tab_p;
-            store_rows_f32(o.p_flat(), 1, c.Fp, 0u, tid, NT, [&](int, int j) { return flat_value(shf, shf, hist, hoff, 0, sh_full, tp[j]); });
+            store_rows(o.p_flat<OT>(), 1, c.Fp, 0u, tid, NT, [&](int, int j) { return flat_value(shf, shf, hist, hoff, 0, sh_full, tp[j]); });
         }
         // agents' flat vectors: sorted-key concatenation
-        store_rows_f32(o.a_flat(), A, c.Fa, c.Fa_magic, tid, NT, [&](int a, int j) {
+        store_rows(o.a_flat<OT>(), A, c.Fa, c.Fa_magic, tid, NT, [&](int a, int j) {
             return flat_value(shf, s.sc_a + a * AS_COUNT, hist, hoff, a * P, sh_full, tab[j]);
         });
         {   // action masks: entry (slot, idx) is open iff idx < limit[agent][slot]
             const uint16_t *mt = tab + c.tab_m;
-            store_rows_f32(o.a_mask(), A, c.Na, c.Na_magic, tid, NT, [&](int a, int j) {
+            store_rows(o.a_mask<OT>(), A, c.Na, c.Na_magic, tid, NT, [&](int a, int j) {
                 const uint32_t en = mt[j];
                 return ((en & 255u) < s.lim[a * MS_COUNT + (en >> 8)]) ? 1.0f : 0.0f;
             });
         }
         if (!EXT || c.Fpa > 0) {   // the planner's per-agent vectors p<i>
             const uint16_t *tpa = tab + c.tab_pa;
-            store_rows_f32(o.p_agents(), A, c.Fpa, c.Fpa_magic, tid, NT, [&](int a, int j) {
+            store_rows(o.p_agents<OT>(), A, c.Fpa, c.Fpa_magic, tid, NT, [&](int a, int j) {
                 return flat_value(shf, s.sc_a + a * AS_COUNT, hist, hoff, a * P, sh_full, tpa[j]);
             });
         }
@@ -509,10 +640,10 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
                 if (open && rr != 0 && c.tax_annealing) open = fabs(c.disc_rates[rr - 1]) <= s.net_hist[2 * P];
                 // single-action planner: one leading NO-OP, then every bracket's R rates (base_agent.py:452-459)
                 const int at = (EXT && c.planner_single) ? (rr == 0 ? 0 : b * c.R + rr) : x;
-                o.p_mask()[at] = open ? 1.0f : 0.0f;
+                put_out(o.p_mask<OT>() + at, open ? 1.0f : 0.0f);
             }
         } else if (tid == 0) {
-            o.p_mask()[0] = 1.0f;
+            put_out(o.p_mask<OT>(), 1.0f);
         }
         if (o.b->policy_seed) {   // the next step's random actions, from the limits / conditions the masks were written from
             const uint64_t key0 = obs_mix64(o.b->policy_seed ^ obs_mix64((uint64_t)o.env)) + ((uint64_t)(uint32_t)e.hdr[HDR_T] << 20) +
@@ -565,13 +696,13 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
     }
     if (c.planner_spatial) {
         int head = 0;
-        const int nwords = bits_words_for(o.p_map(), M * HW, &head);
+        const int nwords = bits_words_for(o.p_map<OT>(), M * HW, &head);
         ex([&](int tid) {
             concat_planes(s.bits, nwords, head, s.pl, psp, M, HW, c.HW_magic, tid, NT);
             store_bytes_i16<true>(o.p_idx(), HW, (const uint8_t *)e.owner, tid, NT);
             store_bytes_i16<false>(o.p_idx() + HW, HW, s.locmap, tid, NT);
         });
-        ex([&](int tid) { stream_bits_f32(o.p_map(), M * HW, s.bits, lut, s.pl, psp, HW, c.HW_magic, tid, NT); });
+        ex([&](int tid) { stream_bits(o.p_map<OT>(), M * HW, s.bits, lut, s.pl, psp, HW, c.HW_magic, tid, NT); });
     }
     if (EXT && c.full_obs) {
         // full_observability (layout_from_file.py:465-472): every agent gets the whole map - the same M bit planes as
@@ -579,7 +710,7 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
         const int HW4 = (HW + 3) & ~3;
         uint8_t *so = s.wi, *sl = s.wi + HW4;
         for (int a = 0; a < A; a++) {
-            float *am = o.b->a_map + (o.env * A + a) * (size_t)c.a_map_elems;
+            OT *am = (OT *)o.b->a_map + (o.env * A + a) * (size_t)c.a_map_elems;
             int16_t *ai = o.b->a_idx + (o.env * A + a) * (size_t)c.a_idx_elems;
             int head = 0;
             const int nwords = bits_words_for(am, M * HW, &head);
@@ -592,7 +723,7 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
                 }
             });
             ex([&](int tid) {
-                stream_bits_f32(am, M * HW, s.bits, lut, s.pl, psp, HW, c.HW_magic, tid, NT);
+                stream_bits(am, M * HW, s.bits, lut, s.pl, psp, HW, c.HW_magic, tid, NT);
                 store_bytes_i16<false>(ai, HW, so, tid, NT);
                 store_bytes_i16<false>(ai + HW, HW, sl, tid, NT);
             });
@@ -608,7 +739,7 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
     const int psa = c.pl_stride_a, units = (ww + 7) >> 3, np1 = M + 1;
     for (int a0 = 0; a0 < A; a0 += c.ob_chunk) {
         const int na = (A - a0 < c.ob_chunk) ? A - a0 : c.ob_chunk;
-        float *am = o.a_map() + (size_t)a0 * np1 * ww;
+        OT *am = o.a_map<OT>() + (size_t)a0 * np1 * ww;
         int head = 0;
         const int nwords = bits_words_for(am, na * np1 * ww, &head);
         ex([&](int tid) {
@@ -650,7 +781,7 @@ AIE_DEV void observe_env(const DevCfg &c, uint8_t *rec, uint8_t *grec, uint8_t *
             store_bytes_i16<false>(o.a_idx() + (size_t)a0 * 2 * ww, na * 2 * ww, s.wi, tid, NT);
             concat_planes(s.bits, nwords, head, s.pl, psa, na * np1, ww, c.ww_magic, tid, NT);
         });
-        ex([&](int tid) { stream_bits_f32(am, na * np1 * ww, s.bits, lut, s.pl, psa, ww, c.ww_magic, tid, NT); });
+        ex([&](int tid) { stream_bits(am, na * np1 * ww, s.bits, lut, s.pl, psa, ww, c.ww_magic, tid, NT); });
     }
 }
 

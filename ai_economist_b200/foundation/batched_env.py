@@ -2,7 +2,8 @@
 (base/base_env.py:24-1120), over E env replicas that live on one GPU.
 
 Differences from the reference API (all additive):
-  * new kwargs `n_envs`, `device`, `seeds`, `auto_reset`, `device_reset`;
+  * new kwargs `n_envs`, `device`, `seeds`, `auto_reset`, `device_reset`, `obs_dtype` (torch.float32, the default, or
+    torch.bfloat16: the float observation / mask tensors are written as bfloat16 by the step kernel itself);
   * observations / rewards / done are persistent device tensors with a leading env axis, keyed exactly like
     the reference's dicts ("0".."n-1", "p"; "world-map", "world-idx_map", "flat", "action_mask", "time", "p<i>");
   * `reference_view(e)` re-creates the reference's nested numpy dict for one env (tests / debugging).
@@ -65,7 +66,7 @@ class BatchedFoundationEnv:
                  flatten_masks=True, allow_observation_scaling=True, dense_log_frequency=None,
                  world_dense_log_frequency=50, collate_agent_step_and_reset_data=False, seed=None,
                  n_envs=1, device="cuda:0", seeds=None, auto_reset=True, stepper_factory=None, device_reset=None,
-                 **scenario_kwargs):
+                 obs_dtype=None, **scenario_kwargs):
         # ---- base_env.py:178-366 argument checks ----
         assert isinstance(world_size, (tuple, list)) and len(world_size) == 2
         self.world_size = list(world_size)
@@ -159,6 +160,8 @@ class BatchedFoundationEnv:
                 spec["reset_mode"] = 0
             else:
                 assert spec.get("reset_mode", 0) == 1, "reference-exact device reset is not available for this config"
+        from .._abi import obs_dtype_name
+        spec["obs_dtype"] = obs_dtype_name(obs_dtype)   # "float32" | "bfloat16"
         self._spec = spec
 
         # ---- dense logging (base_env.py:273-283): replica 0, every dense_log_frequency-th episode ----

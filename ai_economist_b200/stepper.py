@@ -7,6 +7,11 @@ import numpy as np
 from . import _abi
 
 
+def bf16_bits_to_float32(a):
+    """float32 values of raw bfloat16 bits (uint16): exact, every bfloat16 is a float32."""
+    return (np.asarray(a).astype(np.uint32) << 16).view(np.float32)
+
+
 class BatchStepper:
     """Backend-agnostic part (buffer bookkeeping + ABI calls).  Subclasses supply allocation.
 
@@ -14,7 +19,8 @@ class BatchStepper:
     the WarpDrive data manager / function manager for the COVID env.
     """
 
-    _DTYPES = {"u8": np.uint8, "i16": np.int16, "i32": np.int32, "f32": np.float32, "f64": np.float64}
+    # "bf16": bfloat16 observations (spec["obs_dtype"] == "bfloat16"); numpy backends hold their raw bits
+    _DTYPES = {"u8": np.uint8, "i16": np.int16, "i32": np.int32, "f32": np.float32, "f64": np.float64, "bf16": np.uint16}
 
     def __init__(self, spec, n_envs, lib, device_index=0, auto_reset=True, event_envs=0):
         self.spec = dict(spec)
@@ -31,21 +37,22 @@ class BatchStepper:
         full = bool(spec.get("full_observability", 0))   # agents see the whole map: [M, H, W] / [2, H, W] per agent
         none = bool(spec.get("scenario_kind", 0) == 1)   # one-step-economy: no spatial observations (zero-size tensors)
         assert d.agent_map_elems == (0 if none else d.n_map_channels * H * W if full else (d.n_map_channels + 1) * d.window ** 2)
+        fo = "bf16" if self.cfg.obs_dtype == _abi.OBS_BF16 else "f32"   # the float observation / mask tensors
         shapes = {
             "state": ("u8", (E, d.state_bytes)), "state0": ("u8", (E, d.state_bytes)),
             "actions_agent": ("i32", (E, A, d.n_act_agent)),
             "actions_planner": ("i32", (E, max(1, d.n_act_planner))),
-            "obs_agent_map": ("f32", (E, A, 0) if none else (E, A, d.n_map_channels, H, W) if full else
+            "obs_agent_map": (fo, (E, A, 0) if none else (E, A, d.n_map_channels, H, W) if full else
                               (E, A, d.n_map_channels + 1, d.window, d.window)),
             "obs_agent_idx": ("i16", (E, A, 0) if none else (E, A, 2, H, W) if full else (E, A, 2, d.window, d.window)),
-            "obs_agent_flat": ("f32", (E, A, d.flat_agent)),
-            "mask_agent": ("f32", (E, A, d.mask_agent)),
-            "obs_planner_map": ("f32", (E, d.n_map_channels, H, W)),
+            "obs_agent_flat": (fo, (E, A, d.flat_agent)),
+            "mask_agent": (fo, (E, A, d.mask_agent)),
+            "obs_planner_map": (fo, (E, d.n_map_channels, H, W)),
             "obs_planner_idx": ("i16", (E, 2, H, W)),
-            "obs_planner_flat": ("f32", (E, d.flat_planner)),
-            "obs_planner_agents": ("f32", (E, A, d.flat_planner_agent)),
-            "mask_planner": ("f32", (E, d.mask_planner)),
-            "obs_time": ("f32", (E,)),
+            "obs_planner_flat": (fo, (E, d.flat_planner)),
+            "obs_planner_agents": (fo, (E, A, d.flat_planner_agent)),
+            "mask_planner": (fo, (E, d.mask_planner)),
+            "obs_time": (fo, (E,)),
             "reward": ("f64", (E, A + 1)),
             "done": ("i32", (E,)),
         }
@@ -61,6 +68,7 @@ class BatchStepper:
         if self.event_envs:
             shapes["events"] = ("i32", (self.event_envs, self.event_cap + 1, 8))
         self.buf = {k: self._alloc(shape, dt) for k, (dt, shape) in shapes.items()}
+        self._bf16 = {k for k, (dt, _) in shapes.items() if dt == "bf16"}
         bufs = _abi.AieBuffers()
         for name in _abi._BUF_NAMES:
             ok = name in self.buf and int(np.prod(self.buf[name].shape)) > 0   # zero-size tensors have no storage
@@ -287,9 +295,14 @@ class BatchStepper:
             raise _abi.AieError("event log overflow: %d events dropped (capacity %d)" % (dropped, self.event_cap))
         return [tuple(int(v) for v in blk[1 + i]) for i in range(n)]
 
+    def obs_to_numpy(self, name, e=None):
+        """Host copy of output buffer `name` (of env e), bfloat16 observations upcast to float32 (exact)."""
+        a = self.to_numpy(self.buf[name] if e is None else self.buf[name][e])
+        return bf16_bits_to_float32(a) if name in self._bf16 and np.asarray(a).dtype == np.uint16 else a
+
     def read_obs(self, e):
-        """Host copy of env e's outputs in the oracle's obs layout (tests)."""
-        g = lambda k: self.to_numpy(self.buf[k][e]) if k in self.buf else None
+        """Host copy of env e's outputs in the oracle's obs layout (tests); float observations as float32."""
+        g = lambda k: self.obs_to_numpy(k, e) if k in self.buf else None
         out = dict(a_map=g("obs_agent_map"), a_idx=g("obs_agent_idx"), a_flat=g("obs_agent_flat"),
                    a_mask=g("mask_agent"), p_flat=g("obs_planner_flat"), p_agents=g("obs_planner_agents"),
                    p_mask=g("mask_planner"), time=np.atleast_1d(g("obs_time")), rew=g("reward"),
@@ -319,15 +332,15 @@ class CudaStepper(BatchStepper):
         with torch.cuda.device(self.device):
             super().__init__(spec, n_envs, lib, device_index=idx, auto_reset=auto_reset, event_envs=event_envs)
 
-    def _alloc(self, shape, dt):
+    def _torch_dtype(self, dt):
         t = self.torch
-        m = {"u8": t.uint8, "i16": t.int16, "i32": t.int32, "f32": t.float32, "f64": t.float64}
-        return t.zeros(shape, dtype=m[dt], device=self.device)
+        return {"u8": t.uint8, "i16": t.int16, "i32": t.int32, "f32": t.float32, "f64": t.float64, "bf16": t.bfloat16}[dt]
+
+    def _alloc(self, shape, dt):
+        return self.torch.zeros(shape, dtype=self._torch_dtype(dt), device=self.device)
 
     def _empty(self, shape, dt):
-        t = self.torch
-        m = {"u8": t.uint8, "i16": t.int16, "i32": t.int32, "f32": t.float32, "f64": t.float64}
-        return t.empty(shape, dtype=m[dt], device=self.device)
+        return self.torch.empty(shape, dtype=self._torch_dtype(dt), device=self.device)
 
     def _is_f64_contiguous(self, buf):
         t = self.torch
@@ -340,6 +353,8 @@ class CudaStepper(BatchStepper):
         return C.c_void_p(self.torch.cuda.current_stream(self.device).cuda_stream)
 
     def to_numpy(self, buf):
+        if buf.dtype == self.torch.bfloat16:   # numpy has no bfloat16: float32 holds every value exactly
+            buf = buf.float()
         return buf.detach().cpu().numpy()
 
     def state_view(self, name, final=False):

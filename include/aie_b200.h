@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define AIE_ABI_VERSION 4
+#define AIE_ABI_VERSION 5
 
 #define AIE_MAX_COMPONENTS 8
 #define AIE_MAX_BRACKETS 16
@@ -157,7 +157,14 @@ typedef struct aie_config {
     int32_t mz_zones[3];            /* MultiZone: number of Wood, Stone and WoodStone zones */
     int32_t labor_mask_first_step;  /* SimpleLabor mask_first_step: every labor action masked in the reset observation */
     double labor_skill_scale;       /* SimpleLabor payment_max_skill_multiplier: the skill observation is skill / this */
+    /* ABI 5.  Element type of the float observation / mask tensors (obs_agent_map, obs_agent_flat, mask_agent,
+     * obs_planner_map, obs_planner_flat, obs_planner_agents, mask_planner, obs_time): AIE_OBS_F32 (default), or
+     * AIE_OBS_BF16 - every element is the round-to-nearest-even bfloat16 of the float32 the default writes, converted in
+     * the observation pass (half the bytes, no extra pass).  Index planes, rewards, done, state and actions are unchanged.
+     * aie_step_host / aie_step_host_compact take float32 configs only (AIE_EINVAL otherwise). */
+    int32_t obs_dtype;
 } aie_config;
+enum { AIE_OBS_F32 = 0, AIE_OBS_BF16 = 1 };
 
 /* Sizes the caller needs to allocate the device buffers. */
 typedef struct aie_dims {
@@ -172,7 +179,8 @@ typedef struct aie_dims {
     int32_t n_act_agent;      /* ints per agent per step (1 single-action, #subspaces multi-action) */
     int32_t n_act_planner;    /* ints per env per step for the planner (n_brackets, 1 for a single-action planner, or 0) */
     int32_t state_bytes;      /* bytes per env of the packed state record (multiple of 16) */
-    int32_t algorithmic_bytes_per_env_step; /* SURVEY 8(d): obs+mask+rew/done out + actions in + 2*state */
+    int32_t algorithmic_bytes_per_env_step; /* SURVEY 8(d): obs+mask+rew/done out + actions in + 2*state (observation
+                                               bytes at the config's obs_dtype) */
     /* episode statistics ("stats" field of the state record, float64[n_stats], zero at reset): the accumulators
      * behind the reference's component get_metrics() (build.py:198-222, continuous_double_auction.py:585-641,
      * redistribution.py:1141-1186).  Layout: [0] executed trades; [1 + a] houses built by agent a;
@@ -192,7 +200,9 @@ typedef struct aie_dims {
  *   actions_planner: int32 [E, n_act_planner]         may be NULL when n_act_planner == 0
  *   obs_*         : what the reference's step returns per agent key (base_env.py:614-704),
  *                   stacked over envs:  "world-map", "world-idx_map", "flat", "action_mask", "time",
- *                   and for the planner "p<i>" vectors stacked as [E, A, flat_planner_agent]
+ *                   and for the planner "p<i>" vectors stacked as [E, A, flat_planner_agent].
+ *                   With aie_config::obs_dtype == AIE_OBS_BF16 the float* observation / mask pointers below point to
+ *                   bfloat16 storage (2 bytes per element, same shapes)
  *   reward        : float64 [E, A+1]                  agents then planner (layout_from_file.py:519-559)
  *   done          : int32 [E]                         done["__all__"] (base_env.py:1012) */
 typedef struct aie_buffers {
