@@ -114,6 +114,13 @@ class AieHostOut(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in _OUT_NAMES]
 
 
+OBS_NAMES = _OUT_NAMES[:10]   # the observation / mask tensors (aie_obs_buffers)
+
+
+class AieObsBuffers(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in OBS_NAMES]
+
+
 class AieCovidConfig(C.Structure):
     _fields_ = ([(n, C.c_int32) for n in [
         "abi_version", "n_states", "episode_length", "num_stringency_levels", "action_cooldown_period",
@@ -170,6 +177,8 @@ def load_library(path=None):
     L.aie_reset_envs.restype = C.c_int
     L.aie_step.argtypes = [P, P]
     L.aie_observe.argtypes = [P, P]
+    L.aie_observe_final.argtypes = [P, C.POINTER(AieObsBuffers), P]
+    L.aie_observe_final.restype = C.c_int
     L.aie_step_dynamics.argtypes = [P, P]
     L.aie_sample_random_actions.argtypes = [P, C.c_uint64, P]
     L.aie_set_fused_policy.argtypes = [P, C.c_uint64, P]
@@ -210,8 +219,8 @@ def load_library(path=None):
 
 
 EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field", "aie_get_flat_layout", "aie_bind_buffers",
-                    "aie_load_state", "aie_reset_envs", "aie_step", "aie_step_dynamics", "aie_observe", "aie_sample_random_actions", "aie_set_fused_policy",
-                    "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
+                    "aie_load_state", "aie_reset_envs", "aie_step", "aie_step_dynamics", "aie_observe", "aie_observe_final", "aie_sample_random_actions",
+                    "aie_set_fused_policy", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
                     "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
                     "aie_covid_sample_random_actions", "aie_covid_launch_count"]

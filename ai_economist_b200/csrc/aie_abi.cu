@@ -9,6 +9,9 @@
 //   aie_finish_reset_kernel  one warp per env: tax trackers + utility metric_0 after a host reset upload.
 //   aie_reset_kernel       one warp per env: explicit reset on the device (aie_reset_envs), the auto-reset's re-draws.
 //   aie_metrics_kernel     one warp per env: env.metrics from the record in global memory, one row of a float64 table.
+//   aie_observe_final_kernel  one CTA of four warps per env: the stand-alone observation pass over the episode_final
+//                          record of an env whose done flag is set, into the caller's tensors (aie_observe_final); the
+//                          CTAs of the other envs exit early.
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
 // aie_config::obs_dtype == AIE_OBS_BF16); the launchers pick one from the config, with the same launch shape.
 #include <cuda_runtime.h>
@@ -38,6 +41,7 @@ struct State {
     size_t step_smem;    // dynamic shared memory per CTA
     int obs_threads;
     size_t obs_smem;
+    size_t env_cta_smem;   // one env per CTA (aie_observe_final_kernel): shared memory of that CTA
     uint16_t *tab_dev;   // observation programs (device copy)
     uint8_t *compact_dev = nullptr, *compact_host = nullptr;   // aie_step_host_compact: device + pinned host staging
     size_t compact_bytes = 0, compact_host_bytes = 0;
@@ -73,6 +77,7 @@ int launch_reset(aie_env *, const ResetSrc &s, int lo, int n, void *stream);
 int launch_step(aie_env *, int emit_obs, void *stream);
 int launch_step_range(aie_env *, int emit_obs, int lo, int hi, void *stream);
 int launch_observe(aie_env *, int lo, int n, void *stream);
+int launch_observe_final(aie_env *, const DevBufs &fb, void *stream);
 int launch_metrics(aie_env *, int source, double *out, void *stream);
 int launch_sample(aie_env *, uint64_t seed, void *stream);
 int compact_buffers(aie_env *, size_t bytes, uint8_t **dev, uint8_t **host);
@@ -200,6 +205,10 @@ __device__ __noinline__ void auto_reset_env(const DevCfg &c, const DevBufs &b, i
         const uint4 *src = (const uint4 *)(grec + c.off_stats);
         uint4 *dst = (uint4 *)(b.final + (size_t)env * c.rec_bytes + c.off_stats);
         for (int i = lane; i < (8 * c.n_stats + 15) / 16; i += 32) dst[i] = src[i];
+        // so does the price history, which the final observation pass (aie_observe_final_kernel) reads
+        const uint4 *ph = (const uint4 *)(grec + c.off_price_hist);
+        uint4 *ph_dst = (uint4 *)(b.final + (size_t)env * c.rec_bytes + c.off_price_hist);
+        for (int i = lane; i < (c.off_orders - c.off_price_hist) / 16; i += 32) ph_dst[i] = ph[i];
     }
     __syncwarp();
     if (lane == 0) {
@@ -455,10 +464,13 @@ template <bool EXT>
 __global__ void __launch_bounds__(256) aie_observe_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
     observe_kernel_body<EXT, bf16_t>(c, b, lo, n);
 }
-template <bool EXT, typename OT>
+// FINAL (aie_observe_final_kernel): b's record source is episode_final and its outputs are the caller's final tensors;
+// a CTA whose env's done flag is zero leaves before it loads anything or writes any output.
+template <bool EXT, typename OT, bool FINAL = false>
 __device__ __forceinline__ void observe_mw_kernel_body(const DevCfg &c, const DevBufs &b, int lo, int n) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int env = lo + blockIdx.x;
+    if constexpr (FINAL) { if (b.done[env] == 0) return; }   // one env per CTA: the whole CTA leaves
     const uint16_t *tab = stage_tables(smem, 1, c, b);
     uint64_t *bar = (uint64_t *)smem;
     uint8_t *rec = warp_region(smem, 1, 0, c);
@@ -475,6 +487,18 @@ __global__ void __launch_bounds__(128, 4) aie_observe_mw_kernel(const __grid_con
 template <bool EXT>
 __global__ void __launch_bounds__(128, 4) aie_observe_mw_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
     observe_mw_kernel_body<EXT, bf16_t>(c, b, lo, n);
+}
+// Final observations (aie_observe_final): the stand-alone pass over the episode_final records of the envs that finished
+// in the latest step, into the caller's tensors (b: a copy of the bound DevBufs with state = final, the outputs swapped
+// and policy_seed = 0, so no actions are drawn).  One CTA of four warps per env, for every config: the few envs that
+// finish in a staggered step are observed with four warps each (DESIGN.md §6 has the measurement against one warp per env).
+template <bool EXT>
+__global__ void __launch_bounds__(128, 4) aie_observe_final_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+    observe_mw_kernel_body<EXT, float, true>(c, b, lo, n);
+}
+template <bool EXT>
+__global__ void __launch_bounds__(128, 4) aie_observe_final_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
+    observe_mw_kernel_body<EXT, bf16_t, true>(c, b, lo, n);
 }
 
 // Episode metrics (aie_metrics.cuh): one warp per env, eight per CTA, reads the env's record (current or end-of-episode
@@ -566,6 +590,7 @@ int init(aie_env *env) {
     env->be.step_smem = cta_smem(wpb);
     env->be.obs_threads = wpb * 32;
     env->be.obs_smem = env->be.step_smem;
+    env->be.env_cta_smem = cta_smem(1);
     // Register budget: the 64-register variant (launch bounds 256 x 4) when more than 24 warps can be resident (c2: 32
     // warps per SM), otherwise the 80-register variant (c3: 20 warps).  Override: AIE_STEP_MINB=3|4.  Measured on an
     // H100 80GB HBM3 (700 W), one 300-step run per setting, step kernel: c2 248 us with 64 registers vs 305 us with 80;
@@ -605,6 +630,8 @@ int init(aie_env *env) {
     AIE_OPT_IN((aie_step_mw_bf16_kernel<true, false>)); AIE_OPT_IN((aie_step_mw_bf16_kernel<true, true>));
     AIE_OPT_IN(aie_observe_bf16_kernel<false>); AIE_OPT_IN(aie_observe_bf16_kernel<true>);
     AIE_OPT_IN(aie_observe_mw_bf16_kernel<false>); AIE_OPT_IN(aie_observe_mw_bf16_kernel<true>);
+    AIE_OPT_IN(aie_observe_final_kernel<false>); AIE_OPT_IN(aie_observe_final_kernel<true>);
+    AIE_OPT_IN(aie_observe_final_bf16_kernel<false>); AIE_OPT_IN(aie_observe_final_bf16_kernel<true>);
 #undef AIE_OPT_IN
     {
         AIE_CUDA(cudaMalloc((void **)&env->be.tab_dev, sizeof(Tables)), "cudaMalloc tables");
@@ -807,6 +834,20 @@ int launch_observe(aie_env *env, int lo, int n, void *stream) {
     else AIE_OBSERVE(aie_observe_kernel, aie_observe_mw_kernel);
 #undef AIE_OBSERVE
     AIE_CUDA(cudaGetLastError(), "aie_observe_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+// One launch, one CTA of four warps per env; the CTAs of envs whose done flag is zero exit at once.
+int launch_observe_final(aie_env *env, const DevBufs &fb, void *stream) {
+    const int n = env->n_envs;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t sm = env->be.env_cta_smem;
+    if (env->cfg.obs_bf16) {
+        if (env->cfg.ext) aie_observe_final_bf16_kernel<true><<<n, 128, sm, st>>>(env->cfg, fb, 0, n);
+        else aie_observe_final_bf16_kernel<false><<<n, 128, sm, st>>>(env->cfg, fb, 0, n);
+    } else if (env->cfg.ext) aie_observe_final_kernel<true><<<n, 128, sm, st>>>(env->cfg, fb, 0, n);
+    else aie_observe_final_kernel<false><<<n, 128, sm, st>>>(env->cfg, fb, 0, n);
+    AIE_CUDA(cudaGetLastError(), "aie_observe_final_kernel launch");
     env->launches++;
     return AIE_OK;
 }

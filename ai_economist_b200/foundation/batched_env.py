@@ -3,7 +3,9 @@
 
 Differences from the reference API (all additive):
   * new kwargs `n_envs`, `device`, `seeds`, `auto_reset`, `device_reset`, `obs_dtype` (torch.float32, the default, or
-    torch.bfloat16: the float observation / mask tensors are written as bfloat16 by the step kernel itself);
+    torch.bfloat16: the float observation / mask tensors are written as bfloat16 by the step kernel itself),
+    `final_obs` (with auto_reset: `env.final_obs` holds the observations of the state each episode that ended in the
+    latest step ended in, for bootstrapping the value of a truncated episode);
   * observations / rewards / done are persistent device tensors with a leading env axis, keyed exactly like
     the reference's dicts ("0".."n-1", "p"; "world-map", "world-idx_map", "flat", "action_mask", "time", "p<i>");
   * `reference_view(e)` re-creates the reference's nested numpy dict for one env (tests / debugging).
@@ -66,8 +68,11 @@ class BatchedFoundationEnv:
                  flatten_masks=True, allow_observation_scaling=True, dense_log_frequency=None,
                  world_dense_log_frequency=50, collate_agent_step_and_reset_data=False, seed=None,
                  n_envs=1, device="cuda:0", seeds=None, auto_reset=True, stepper_factory=None, device_reset=None,
-                 obs_dtype=None, **scenario_kwargs):
+                 obs_dtype=None, final_obs=False, **scenario_kwargs):
         # ---- base_env.py:178-366 argument checks ----
+        if final_obs and not auto_reset:
+            raise ValueError("final_obs=True needs auto_reset=True: without the auto-reset, env.obs after the step that "
+                             "ends an episode already is its final observation")
         assert isinstance(world_size, (tuple, list)) and len(world_size) == 2
         self.world_size = list(world_size)
         assert isinstance(n_agents, int) and n_agents >= 2
@@ -162,6 +167,7 @@ class BatchedFoundationEnv:
                 assert spec.get("reset_mode", 0) == 1, "reference-exact device reset is not available for this config"
         from .._abi import obs_dtype_name
         spec["obs_dtype"] = obs_dtype_name(obs_dtype)   # "float32" | "bfloat16"
+        spec["final_obs"] = bool(final_obs)
         self._spec = spec
 
         # ---- dense logging (base_env.py:273-283): replica 0, every dense_log_frequency-th episode ----
@@ -584,6 +590,27 @@ class BatchedFoundationEnv:
         b = self._stepper.buf
         A = self.n_agents
         self.obs_tensors = {k: b[k] for k in b if k.startswith("obs_") or k.startswith("mask_")}
+        self.obs = self._obs_views(b)
+        self.rew = {str(i): b["reward"][:, i] for i in range(A)}
+        self.rew["p"] = b["reward"][:, A]
+        self.done = {"__all__": b["done"]}
+        self.info = {k: {} for k in self.obs}
+        if self.collate_agent_step_and_reset_data:
+            self.rew = {"a": b["reward"][:, :A], "p": b["reward"][:, A]}
+            self.info = {"a": {str(i): {} for i in range(A)}, "p": {}}
+        # final_obs=True: env.final_obs / env.final_obs_tensors mirror env.obs / env.obs_tensors over the final_<name>
+        # buffers.  After a step, row e of a replica with done["__all__"][e] == 1 holds the observation of the state its
+        # episode ended in (env.obs already shows the next episode's first); the other rows are unspecified (they keep
+        # whatever an earlier episode end wrote).  reset() does not touch them.  None when final_obs is off.
+        self.final_obs_tensors = self.final_obs = None
+        if getattr(self._stepper, "final_obs", False):
+            self.final_obs_tensors = {k: b["final_" + k] for k in self.obs_tensors}
+            self.final_obs = self._obs_views(self.final_obs_tensors)
+
+    def _obs_views(self, b):
+        """The nested observation dict (keys and views as the reference's step returns them) over the observation / mask
+        buffers `b` (name -> tensor): the live ones, or their final_<name> twins."""
+        A = self.n_agents
         flat_o, flat_m = self._flatten_observations, self._flatten_masks
         if not flat_o:
             st = self._stepper
@@ -612,10 +639,6 @@ class BatchedFoundationEnv:
             p["p%d" % i] = b["obs_planner_agents"][:, i] if flat_o else \
                 self._named_fields(b["obs_planner_agents"][:, i], lay_pa)
         obs["p"] = p
-        self.rew = {str(i): b["reward"][:, i] for i in range(A)}
-        self.rew["p"] = b["reward"][:, A]
-        self.done = {"__all__": b["done"]}
-        self.info = {k: {} for k in obs}
         if self.collate_agent_step_and_reset_data:
             # base_env.py:816-850: the agents' entries are stacked under "a" with the agent axis LAST
             # ([E, ..., A]); these are strided views of the same [E, A, ...] device tensors, no copy
@@ -629,9 +652,7 @@ class BatchedFoundationEnv:
                    "p": obs["p"]}
             if spatial:
                 obs["a"].update({"world-map": last(b["obs_agent_map"]), "world-idx_map": last(b["obs_agent_idx"])})
-            self.rew = {"a": b["reward"][:, :A], "p": b["reward"][:, A]}
-            self.info = {"a": {str(i): {} for i in range(A)}, "p": {}}
-        self.obs = obs
+        return obs
 
     def reference_view(self, e=0):
         """(obs, rew, done) of env e as nested numpy dicts in the reference's layout."""

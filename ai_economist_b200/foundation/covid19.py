@@ -221,10 +221,12 @@ class CovidBatchedEnv:
                  flatten_masks=True, collate_agent_step_and_reset_data=True, allow_observation_scaling=True,
                  use_real_world_data=False, use_real_world_policies=False, n_envs=1, device="cuda:0", auto_reset=True,
                  stepper_factory=None, seed=None, seeds=None, dense_log_frequency=None, world_dense_log_frequency=50,
-                 obs_dtype=None, **scenario_kwargs):
+                 obs_dtype=None, final_obs=False, **scenario_kwargs):
         from .._abi import obs_dtype_name
         if obs_dtype_name(obs_dtype) != "float32":
             raise NotImplementedError("the COVID-19 scenario writes float32 observations only")
+        if final_obs:
+            raise NotImplementedError("final_obs is not available for the COVID-19 scenario")
         assert collate_agent_step_and_reset_data, \
             "The env. config 'collate_agent_step_and_reset_data' should be set to True."
         if use_real_world_data or use_real_world_policies:

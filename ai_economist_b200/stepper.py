@@ -60,6 +60,13 @@ class BatchStepper:
             shapes["episode_final"] = ("u8", (E, d.state_bytes))
         if not spec["planner_gets_spatial_info"]:
             del shapes["obs_planner_map"], shapes["obs_planner_idx"]
+        # spec["final_obs"]: final_<name> twins of the observation / mask buffers, written by step() for the replicas
+        # whose episode the auto-reset ended (aie_observe_final)
+        self.final_obs = bool(spec.get("final_obs", False))
+        if self.final_obs and not auto_reset:
+            raise ValueError("final_obs needs auto_reset: without it the observations of the ending step are the final ones")
+        if self.final_obs:
+            shapes.update({"final_" + k: shapes[k] for k in _abi.OBS_NAMES if k in shapes})
         # per-step event log of the first event_envs replicas (dense logs): capacity = every agent builds, gathers both
         # resources and every resting order trades
         self.event_envs = max(0, min(int(event_envs), E))
@@ -77,6 +84,10 @@ class BatchStepper:
         bufs.event_envs, bufs.event_cap = self.event_envs, self.event_cap
         self._check(lib.aie_bind_buffers(self._h, C.byref(bufs)))
         self._fields = {}
+        self._final_out = self._final_bufs = None
+        if self.final_obs:   # the default destination of observe_final, built once (step() launches into it every step)
+            self._final_out = {k: self.buf["final_" + k] for k in _abi.OBS_NAMES if k in self.buf}
+            self._final_bufs = self._obs_buffers(self._final_out)
 
     # -- to be provided by subclasses ------------------------------------------------------------------
     def _alloc(self, shape, dt):
@@ -203,11 +214,49 @@ class BatchStepper:
         self._check(self.lib.aie_reset_envs(self._h, tmpl, rs, int(env_lo), n, self._stream()))
 
     def step(self):
-        """Advance every env by one timestep from the bound action buffers (asynchronous on the stream)."""
+        """Advance every env by one timestep from the bound action buffers (asynchronous on the stream); with final_obs,
+        then write the final observations of the episodes that ended into the final_<name> buffers."""
         self._check(self.lib.aie_step(self._h, self._stream()))
+        if self.final_obs:
+            self.observe_final()
 
     def observe(self):
         self._check(self.lib.aie_observe(self._h, self._stream()))
+
+    def observe_final(self, out=None):
+        """Observations / masks of the state each episode that ended in the latest step ended in (its episode_final
+        record), into row e of every replica e whose done flag is set; other rows are left as they are (aie_observe_final,
+        one launch, asynchronous on the stream; needs auto_reset).  out: None (the final_<name> buffers) or a dict
+        name -> buffer for every observation / mask buffer of the stepper (same shape and dtype, contiguous), e.g. a
+        trainer's rollout slot.  Returns the dict written to."""
+        if out is None:
+            if not self.final_obs:
+                raise _abi.AieError("observe_final: no final_<name> buffers (final_obs is off); pass out=")
+            out, o = self._final_out, self._final_bufs
+        else:
+            for k in _abi.OBS_NAMES:
+                if k not in self.buf:
+                    continue
+                if k not in out:
+                    raise _abi.AieError("observe_final: out has no %s buffer" % k)
+                if not self._same_layout(out[k], self.buf[k]):
+                    raise _abi.AieError("observe_final: out[%r] must be a contiguous %s %s buffer on the stepper's device"
+                                        % (k, self.buf[k].dtype, tuple(self.buf[k].shape)))
+            o = self._obs_buffers(out)
+        self._check(self.lib.aie_observe_final(self._h, C.byref(o), self._stream()))
+        return out
+
+    def _obs_buffers(self, out):
+        """aie_obs_buffers over the buffers of `out` (zero-size tensors have no storage: NULL)."""
+        o = _abi.AieObsBuffers()
+        for k in _abi.OBS_NAMES:
+            if k in self.buf and int(np.prod(self.buf[k].shape)) > 0:
+                setattr(o, k, self._ptr(out[k]))
+        return o
+
+    def _same_layout(self, buf, like):
+        return (isinstance(buf, np.ndarray) and buf.dtype == like.dtype and buf.shape == like.shape
+                and buf.flags["C_CONTIGUOUS"])
 
     def step_dynamics(self):
         self._check(self.lib.aie_step_dynamics(self._h, self._stream()))
@@ -345,6 +394,11 @@ class CudaStepper(BatchStepper):
     def _is_f64_contiguous(self, buf):
         t = self.torch
         return isinstance(buf, t.Tensor) and buf.dtype == t.float64 and buf.is_contiguous() and buf.device == self.device
+
+    def _same_layout(self, buf, like):
+        t = self.torch
+        return (isinstance(buf, t.Tensor) and buf.dtype == like.dtype and buf.shape == like.shape and buf.is_contiguous()
+                and buf.device == self.device)
 
     def _ptr(self, buf):
         return C.c_void_p(buf.data_ptr())

@@ -361,6 +361,23 @@ int aie_step(aie_env *env, void *stream);
 int aie_step_dynamics(aie_env *env, void *stream);
 int aie_observe(aie_env *env, void *stream);
 
+/* The ten observation / mask tensors of aie_buffers, with the same shapes and element types (the float pointers point to
+ * bfloat16 storage when obs_dtype == AIE_OBS_BF16); the same pointers are required as by aie_bind_buffers. */
+typedef struct aie_obs_buffers {
+    float *obs_agent_map; int16_t *obs_agent_idx; float *obs_agent_flat; float *mask_agent;
+    float *obs_planner_map; int16_t *obs_planner_idx; float *obs_planner_flat; float *obs_planner_agents;
+    float *mask_planner; float *obs_time;
+} aie_obs_buffers;
+
+/* ABI 5.  Final observations of the episodes the auto-reset ended: for every env whose done flag is non-zero after the
+ * latest aie_step, writes the observations / masks of its episode_final record (the state its episode ended in, which
+ * the step's own outputs no longer show: they belong to the new episode) into row e of `out`; every other row is left
+ * untouched.  What a trainer bootstraps a truncated episode's value from (gymnasium's final_obs).  One launch,
+ * asynchronous on `stream`; draws no actions, even with the fused policy on.  AIE_EINVAL for a NULL out, a missing
+ * required pointer or a pointer not aligned to its element size; AIE_ESTATE before buffers are bound and state is
+ * loaded, or without episode_final records (no episode_final buffer bound, or auto_reset off). */
+int aie_observe_final(aie_env *env, const aie_obs_buffers *out, void *stream);
+
 /* Random policy on the device: writes into the bound action buffers one uniformly random *unmasked* action
  * per agent (per subspace in multi-action mode) and per planner bracket, from the current mask tensors.
  * Replaces: BaseAgent.get_random_action / populate_random_actions (base/base_agent.py:365-405) and the
