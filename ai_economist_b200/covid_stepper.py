@@ -4,6 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
+from .stepper import PolicySampler, buf_kind_torch
 
 F32, I32 = np.float32, np.int32
 
@@ -67,7 +68,7 @@ def covid_config_from_params(p, auto_reset=True):
     return cfg, keep
 
 
-class CovidStepperBase:
+class CovidStepperBase(PolicySampler):
     _DT = {"f32": np.float32, "f64": np.float64, "i32": np.int32, "i8": np.int8}
 
     def __init__(self, params, n_envs, lib, device_index=0, auto_reset=True, change_list=None):
@@ -130,6 +131,16 @@ class CovidStepperBase:
     def sample_random_actions(self, seed=0):
         self._check(self.lib.aie_covid_sample_random_actions(self._h, C.c_uint64(int(seed)), self._stream()))
 
+    # sample_policy (PolicySampler): agent logits [E, S, 1 + levels] (action axis last; the mask is [E, 1 + levels, S]),
+    # planner logits [E, 1 + subsidy levels]; log-probabilities [E, S] and [E]
+    @property
+    def _policy_fn(self):
+        return self.lib.aie_covid_sample_policy
+
+    def _policy_shapes(self):
+        E, S = self.n_envs, self.p["n_states"]
+        return ((E, S, 1 + self.p["num_stringency_levels"]), (E, 1 + self.p["num_subsidy_levels"]), (E, S), (E,))
+
     def launch_count(self):
         return int(self.lib.aie_covid_launch_count(self._h))
 
@@ -167,6 +178,9 @@ class CudaCovidStepper(CovidStepperBase):
         t = self.torch
         m = {"i8": t.int8, "i32": t.int32, "f32": t.float32, "f64": t.float64}
         return t.zeros(shape, dtype=m[dt], device=self.device)
+
+    def _buf_kind(self, buf):
+        return buf_kind_torch(self.torch, self.device, buf)
 
     def _ptr(self, buf):
         return C.c_void_p(buf.data_ptr())

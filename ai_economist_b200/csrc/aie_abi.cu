@@ -12,6 +12,10 @@
 //   aie_observe_final_kernel  one CTA of four warps per env: the stand-alone observation pass over the episode_final
 //                          record of an env whose done flag is set, into the caller's tensors (aie_observe_final); the
 //                          CTAs of the other envs exit early.
+//   aie_sample_policy_kernel  one warp per env, or per (env, unit) for many agent segments: a policy's actions drawn
+//                          from its logits under the current masks (aie_sample_policy), with their log-probabilities;
+//                          *_bf16 reads bfloat16 masks, and each is instantiated for float32 and bfloat16 logits.
+//   aie_covid_sample_policy_kernel  one warp per (env, state | planner): the same for the COVID-19 scenario.
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
 // aie_config::obs_dtype == AIE_OBS_BF16); the launchers pick one from the config, with the same launch shape.
 #include <cuda_runtime.h>
@@ -80,6 +84,7 @@ int launch_observe(aie_env *, int lo, int n, void *stream);
 int launch_observe_final(aie_env *, const DevBufs &fb, void *stream);
 int launch_metrics(aie_env *, int source, double *out, void *stream);
 int launch_sample(aie_env *, uint64_t seed, void *stream);
+int launch_policy(aie_env *, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream);
 int compact_buffers(aie_env *, size_t bytes, uint8_t **dev, uint8_t **host);
 int staging_node(aie_env *);
 int launch_pack_range(aie_env *, const CompactLayout &L, uint8_t *dev, int lo, int hi, void *stream);
@@ -95,6 +100,7 @@ void const_free(void *dev);
 int covid_launch_reset(aie_covid_env *, void *stream);
 int covid_launch_step(aie_covid_env *, void *stream);
 int covid_launch_sample(aie_covid_env *, uint64_t key, void *stream);
+int covid_launch_policy(aie_covid_env *, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream);
 }  // namespace be
 }  // namespace aie
 
@@ -539,6 +545,30 @@ __global__ void __launch_bounds__(256) aie_sample_bf16_kernel(const __grid_const
     sample_kernel_body<EXT, bf16_t>(c, b, seed, per_unit);
 }
 
+// Policy sampler (aie_sample_policy): the random sampler's launch shape (per_unit 0: one warp per env, 1: one warp per
+// (env, unit)); MT: mask element type (the config's obs_dtype), LT: logits element type (the caller's).  Launch bounds
+// (256, 2): without a minimum the EXT instantiations spill 4 bytes at 80 registers; with it they take 95 (the others 80).
+template <bool EXT, typename MT, typename LT>
+__device__ __forceinline__ void policy_kernel_body(const DevCfg &c, const DevBufs &b, const PolicyBufs &p, uint64_t seed,
+                                                   int per_unit) {
+    const long long wid = (long long)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    const int units = per_unit ? c.A + (c.planner_acts ? c.B : 0) : 1;
+    const int env = (int)(wid / units), u = (int)(wid - (long long)env * units);
+    if (env >= c.n_envs) return;
+    policy_actions_env<EXT, MT, LT>(c, b, p, env, mix64(seed ^ mix64((uint64_t)env)), per_unit ? u : -1, lane);
+}
+template <bool EXT, typename LT>
+__global__ void __launch_bounds__(256, 2) aie_sample_policy_kernel(const __grid_constant__ DevCfg c, const DevBufs b,
+                                                                const PolicyBufs p, uint64_t seed, int per_unit) {
+    policy_kernel_body<EXT, float, LT>(c, b, p, seed, per_unit);
+}
+template <bool EXT, typename LT>   // reads bfloat16 masks
+__global__ void __launch_bounds__(256, 2) aie_sample_policy_bf16_kernel(const __grid_constant__ DevCfg c, const DevBufs b,
+                                                                     const PolicyBufs p, uint64_t seed, int per_unit) {
+    policy_kernel_body<EXT, bf16_t, LT>(c, b, p, seed, per_unit);
+}
+
 // ---------------------------------------------------------------------------------------------------------
 namespace be {
 
@@ -880,6 +910,31 @@ int launch_sample(aie_env *env, uint64_t seed, void *stream) {
     return AIE_OK;
 }
 
+// One warp per (env, unit) from this many agent segments per env (agents x subspaces) up, one warp per env below.
+constexpr int POLICY_PER_UNIT_MIN = 64;
+// sd: the call's stream (host_mix64(seed) ^ host_mix64(policy call)); lt_bf16: the logits are bfloat16.
+int launch_policy(aie_env *env, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream) {
+    const DevCfg &c = env->cfg;
+    const int units = c.A + (c.planner_acts ? c.B : 0);
+    int per_unit = (c.A * (c.multi_action ? c.n_sub : 1) >= POLICY_PER_UNIT_MIN) ? 1 : 0;
+    if (const char *v = getenv("AIE_POLICY_PER_UNIT")) per_unit = atoi(v) ? 1 : 0;   // timing aid (tools/time_policy_sampler.py)
+    const long long warps = (long long)env->n_envs * (per_unit ? units : 1);
+    const unsigned grid = (unsigned)((warps + 7) / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+#define AIE_POLICY_LAUNCH(K, LT)                                                                         \
+    (c.ext ? K<true, LT><<<grid, 256, 0, st>>>(c, env->bufs, p, sd, per_unit)                          \
+           : K<false, LT><<<grid, 256, 0, st>>>(c, env->bufs, p, sd, per_unit))
+    if (c.obs_bf16) {
+        if (lt_bf16) AIE_POLICY_LAUNCH(aie_sample_policy_bf16_kernel, bf16_t);
+        else AIE_POLICY_LAUNCH(aie_sample_policy_bf16_kernel, float);
+    } else if (lt_bf16) AIE_POLICY_LAUNCH(aie_sample_policy_kernel, bf16_t);
+    else AIE_POLICY_LAUNCH(aie_sample_policy_kernel, float);
+#undef AIE_POLICY_LAUNCH
+    AIE_CUDA(cudaGetLastError(), "aie_sample_policy_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+
 }  // namespace be
 
 // ---------------------------------------------------------------------------------------------------------
@@ -895,6 +950,16 @@ __global__ void __launch_bounds__(64) aie_covid_reset_kernel(const __grid_consta
 
 __global__ void __launch_bounds__(64) aie_covid_sample_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b, uint64_t key) {
     covid_sample_env(c, blockIdx.x, b, cv_mix64(key ^ cv_mix64(blockIdx.x)), threadIdx.x, blockDim.x);
+}
+// Policy sampler (aie_covid_sample_policy): one warp per (env, unit), units = S states + the planner, eight per CTA.
+template <typename LT>
+__global__ void __launch_bounds__(256) aie_covid_sample_policy_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                      const PolicyBufs p, uint64_t sd) {
+    const long long wid = (long long)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
+    const int units = c.S + 1;
+    const int env = (int)(wid / units), u = (int)(wid - (long long)env * units);
+    if (env >= c.n_envs) return;
+    covid_policy_unit<LT>(c, env, b, p, cv_mix64(sd ^ cv_mix64((uint64_t)env)), u, threadIdx.x & 31);
 }
 
 namespace be {
@@ -920,6 +985,14 @@ int covid_launch_reset(aie_covid_env *env, void *stream) {
 int covid_launch_sample(aie_covid_env *env, uint64_t key, void *stream) {
     aie_covid_sample_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, key);
     AIE_CUDA(cudaGetLastError(), "aie_covid_sample_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+int covid_launch_policy(aie_covid_env *env, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream) {
+    const unsigned grid = (unsigned)(((long long)env->n_envs * (env->cfg.S + 1) + 7) / 8);
+    if (lt_bf16) aie_covid_sample_policy_kernel<bf16_t><<<grid, 256, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, p, sd);
+    else aie_covid_sample_policy_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, p, sd);
+    AIE_CUDA(cudaGetLastError(), "aie_covid_sample_policy_kernel launch");
     env->launches++;
     return AIE_OK;
 }

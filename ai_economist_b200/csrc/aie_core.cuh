@@ -1614,4 +1614,195 @@ AIE_DEV void sample_actions_env(const DevCfg &c, const MT *a_mask, const MT *p_m
     for (int u = 0; u < units; u++) sample_actions_unit<EXT, MT>(c, a_mask, p_mask, act_a, act_p, key, u, lane);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Policy sampler (aie_sample_policy): one categorical draw per mask segment from the softmax of the caller's logits
+// restricted to the open entries.  Random stream: u = (mix64(k) >> 11) * 2^-53 per segment, k the key the random
+// sampler hashes for that segment (sample_actions_unit; the per-env key comes from a call counter of its own).  Draw:
+// m = largest open logit, w_j = exp((double)l_j - m) for open j (0 otherwise), Z = sum w; the action is the smallest
+// j with w_j > 0 and u * Z < w_0 + .. + w_j (float64), else the last j with w_j > 0 (rounding).  greedy: the first
+// open j with l_j == m.  log-prob = (float)(((double)l_a - m) - log(Z)).  No open entry: action 0, log-prob 0; an open
+// logit that is NaN or +inf, or no finite open logit: the first open entry, log-prob NaN.
+// ------------------------------------------------------------------------------------------------
+AIE_DEV float logit_value(float v) { return v; }
+AIE_DEV float logit_value(bf16_t v) {
+#if AIE_ON_DEVICE
+    return __uint_as_float((uint32_t)v.bits << 16);
+#else
+    const uint32_t u = (uint32_t)v.bits << 16;
+    float f;
+    memcpy(&f, &u, 4);
+    return f;
+#endif
+}
+AIE_DEV double policy_uniform(uint64_t key) { return (double)(mix64(key) >> 11) * 0x1.0p-53; }
+
+// One segment: mask[j * ms] (ms: element stride of the mask; 1 except for the COVID agents' [levels][S] masks) and
+// logit[j], j < n <= MAX_MASK.  Returns the action on every lane and writes the log-probability to *lp on every lane.
+// Device: one warp, entry j on lane j % 32 of chunk j / 32 (five chunks); max and prefix by shuffles, crossing by ballot.
+template <typename MT, typename LT>
+AIE_DEV int policy_segment_warp(const MT *mask, int ms, const LT *logit, int n, uint64_t key, int greedy, int lane, float *lp) {
+#if AIE_ON_DEVICE
+    float lv[5];
+    uint32_t om[5], bad = 0, fin = 0, any = 0;
+    float mx = -INFINITY;
+#pragma unroll
+    for (int ch = 0; ch < 5; ch++) {
+        const int j = ch * NL + lane;
+        const bool o = j < n && mask_open(mask[(size_t)j * ms]);
+        const float v = o ? logit_value(logit[j]) : -INFINITY;
+        lv[ch] = v;
+        om[ch] = wballot(o);
+        any |= om[ch];
+        bad |= wballot(o && !(v < INFINITY));          // NaN or +inf
+        fin |= wballot(o && v > -INFINITY && v < INFINITY);
+        mx = fmaxf(mx, v);
+    }
+    if (!any) { *lp = 0.0f; return 0; }
+    if (bad || !fin) {
+        *lp = __int_as_float(0x7fc00000);
+#pragma unroll
+        for (int ch = 0; ch < 5; ch++)
+            if (om[ch]) return ch * NL + first_lane(om[ch]);
+        return 0;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const double m = (double)mx;
+    double cum[5];
+    uint32_t pos[5];
+    double carry = 0.0;
+#pragma unroll
+    for (int ch = 0; ch < 5; ch++) {
+        cum[ch] = 0.0; pos[ch] = 0u;
+        if (ch * NL < n) {   // warp-uniform
+            const double w = ((om[ch] >> lane) & 1u) ? exp((double)lv[ch] - m) : 0.0;
+            pos[ch] = wballot(w > 0.0);
+            double s = w;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const double t = __shfl_up_sync(0xffffffffu, s, o);
+                if (lane >= o) s += t;
+            }
+            cum[ch] = carry + s;
+            carry = __shfl_sync(0xffffffffu, cum[ch], 31);
+        }
+    }
+    const double Z = carry;
+    int a = -1;
+    if (greedy) {
+#pragma unroll
+        for (int ch = 0; ch < 5; ch++) {
+            const uint32_t hit = wballot(((om[ch] >> lane) & 1u) && lv[ch] == mx);
+            if (a < 0 && hit) a = ch * NL + first_lane(hit);
+        }
+    } else {
+        const double t = policy_uniform(key) * Z;
+#pragma unroll
+        for (int ch = 0; ch < 5; ch++) {
+            const uint32_t hit = wballot(((pos[ch] >> lane) & 1u) && t < cum[ch]);
+            if (a < 0 && hit) a = ch * NL + first_lane(hit);
+        }
+        if (a < 0) {
+#pragma unroll
+            for (int ch = 0; ch < 5; ch++)
+                if (pos[ch]) a = ch * NL + 31 - __clz(pos[ch]);
+        }
+    }
+    const double la = greedy ? m : (double)logit_value(logit[a]);
+    *lp = (float)((la - m) - log(Z));
+    return a;
+#else
+    int first = -1;
+    bool bad = false, fin = false;
+    float mx = -INFINITY;
+    for (int j = 0; j < n; j++) {
+        if (!mask_open(mask[(size_t)j * ms])) continue;
+        const float v = logit_value(logit[j]);
+        if (first < 0) first = j;
+        if (!(v < INFINITY)) bad = true;
+        else if (v > -INFINITY) { fin = true; mx = v > mx ? v : mx; }
+    }
+    if (first < 0) { *lp = 0.0f; return 0; }
+    if (bad || !fin) { *lp = NAN; return first; }
+    const double m = (double)mx;
+    double Z = 0.0;
+    for (int j = 0; j < n; j++)
+        if (mask_open(mask[(size_t)j * ms])) Z += exp((double)logit_value(logit[j]) - m);
+    int a = -1;
+    if (greedy) {
+        for (int j = 0; j < n && a < 0; j++)
+            if (mask_open(mask[(size_t)j * ms]) && logit_value(logit[j]) == mx) a = j;
+    } else {
+        const double t = policy_uniform(key) * Z;
+        double cum = 0.0;
+        int last = -1;
+        for (int j = 0; j < n && a < 0; j++) {
+            if (!mask_open(mask[(size_t)j * ms])) continue;
+            const double w = exp((double)logit_value(logit[j]) - m);
+            cum += w;
+            if (w > 0.0) { last = j; if (t < cum) a = j; }
+        }
+        if (a < 0) a = last;
+    }
+    *lp = (float)(((double)logit_value(logit[a]) - m) - log(Z));
+    return a;
+#endif
+}
+
+// Where aie_sample_policy reads and writes (device pointers; the log-probabilities are optional)
+struct PolicyBufs {
+    const void *a_logit, *p_logit;   // [E][A][Na], [E][Np]: float or bf16_t (the kernel's LT)
+    float *lp_a, *lp_p;              // [E][A][n_act_a], [E][n_act_p] or null
+    int32_t greedy;
+};
+
+// One unit of the policy sampler, laid out and keyed like sample_actions_unit (unit u < A: agent u, one draw per
+// subspace; unit A + b: planner bracket b, or the single-action planner's one index).
+template <bool EXT, typename MT, typename LT>
+AIE_DEV void policy_actions_unit(const DevCfg &c, const MT *a_mask, const MT *p_mask, const LT *a_logit, const LT *p_logit,
+                                 int32_t *act_a, int32_t *act_p, float *lp_a, float *lp_p, uint64_t key, int greedy, int u,
+                                 int lane) {
+    float lp;
+    if (u < c.A) {
+        const int a = u;
+        const MT *m = a_mask + (size_t)a * c.Na;
+        const LT *l = a_logit + (size_t)a * c.Na;
+        if (!c.multi_action) {
+            const int v = policy_segment_warp(m, 1, l, c.Na, key + 0x100 * a, greedy, lane, &lp);
+            if (lane == 0) { act_a[a] = v; if (lp_a) lp_a[a] = lp; }
+        } else {
+            int off = 0;
+            for (int si = 0; si < c.n_sub; si++) {
+                const int v = policy_segment_warp(m + off, 1, l + off, c.sub_n[si] + 1, key + 0x100 * a + si + 1, greedy, lane, &lp);
+                if (lane == 0) { act_a[a * c.n_sub + si] = v; if (lp_a) lp_a[a * c.n_sub + si] = lp; }
+                off += c.sub_n[si] + 1;
+            }
+        }
+    } else if (EXT && c.planner_single) {
+        if (u == c.A) {
+            const int v = policy_segment_warp(p_mask, 1, p_logit, c.Np, key + 0x10000, greedy, lane, &lp);
+            if (lane == 0) { act_p[0] = v; if (lp_p) lp_p[0] = lp; }
+        }
+    } else if (c.planner_acts) {
+        const int b = u - c.A;
+        const size_t off = (size_t)b * (1 + c.R);
+        const int v = policy_segment_warp(p_mask + off, 1, p_logit + off, 1 + c.R, key + 0x10000 + b, greedy, lane, &lp);
+        if (lane == 0) { act_p[b] = v; if (lp_p) lp_p[b] = lp; }
+    }
+}
+// Env e's pointers, and every unit of it (u < 0) or unit u only.  key: mix64(s ^ mix64(e)), s the call's stream.
+template <bool EXT, typename MT, typename LT>
+AIE_DEV void policy_actions_env(const DevCfg &c, const DevBufs &b, const PolicyBufs &p, int e, uint64_t key, int u, int lane) {
+    const MT *am = (const MT *)b.a_mask + (size_t)e * c.A * c.Na, *pm = (const MT *)b.p_mask + (size_t)e * c.Np;
+    const LT *al = (const LT *)p.a_logit + (size_t)e * c.A * c.Na;
+    const LT *pl = c.n_act_p ? (const LT *)p.p_logit + (size_t)e * c.Np : nullptr;
+    int32_t *aa = const_cast<int32_t *>(b.act_a) + (size_t)e * c.A * c.n_act_a;
+    int32_t *ap = c.n_act_p ? const_cast<int32_t *>(b.act_p) + (size_t)e * c.n_act_p : nullptr;
+    float *la = p.lp_a ? p.lp_a + (size_t)e * c.A * c.n_act_a : nullptr;
+    float *lq = (p.lp_p && c.n_act_p) ? p.lp_p + (size_t)e * c.n_act_p : nullptr;
+    if (u >= 0) { policy_actions_unit<EXT>(c, am, pm, al, pl, aa, ap, la, lq, key, p.greedy, u, lane); return; }
+    const int units = c.A + (c.planner_acts ? c.B : 0);
+    for (int v = 0; v < units; v++) policy_actions_unit<EXT>(c, am, pm, al, pl, aa, ap, la, lq, key, p.greedy, v, lane);
+}
+
 }  // namespace aie

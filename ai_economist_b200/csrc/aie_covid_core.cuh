@@ -15,6 +15,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "aie_core.cuh"   // policy_segment_warp, PolicyBufs
+
 #if defined(__CUDACC__) && !defined(AIE_EMU)
 #define CV_DEV __device__ __forceinline__
 #define CV_ON_DEVICE 1
@@ -404,6 +406,26 @@ CV_DEV void covid_sample_env(const CovidCfg &c, int e, const CovidBufs &b, uint6
         const bool open = b.mask_p[(size_t)e * (1 + c.sub_levels) + 1] != 0.0f;
         const uint32_t r = (uint32_t)(cv_mix64(key ^ 0xabcdefull) >> 32);
         const_cast<int32_t *>(b.act_p)[e] = open ? (int32_t)(r % (uint32_t)(1 + c.sub_levels)) : 0;
+    }
+}
+
+// Policy sampler (aie_covid_sample_policy, policy_segment_warp in aie_core.cuh): unit u < S draws state u's stringency
+// level from its logits [E][S][1 + levels] under the mask column mask_a[e][.][u]; unit S draws the planner's subsidy
+// level from [E][1 + sub_levels].  Keys as covid_sample_env: key + 0x100 * u for a state, key ^ 0xabcdef for the planner.
+template <typename LT>
+CV_DEV void covid_policy_unit(const CovidCfg &c, int e, const CovidBufs &b, const PolicyBufs &p, uint64_t key, int u, int lane) {
+    float lp;
+    if (u < c.S) {
+        const int n = 1 + c.levels;
+        const size_t i = (size_t)e * c.S + u;
+        const int v = policy_segment_warp(b.mask_a + (size_t)e * n * c.S + u, c.S, (const LT *)p.a_logit + i * n, n,
+                                          key + 0x100 * (uint64_t)u, p.greedy, lane, &lp);
+        if (lane == 0) { const_cast<int32_t *>(b.act_a)[i] = v; if (p.lp_a) p.lp_a[i] = lp; }
+    } else {
+        const int n = 1 + c.sub_levels;
+        const int v = policy_segment_warp(b.mask_p + (size_t)e * n, 1, (const LT *)p.p_logit + (size_t)e * n, n,
+                                          key ^ 0xabcdefull, p.greedy, lane, &lp);
+        if (lane == 0) { const_cast<int32_t *>(b.act_p)[e] = v; if (p.lp_p) p.lp_p[e] = lp; }
     }
 }
 

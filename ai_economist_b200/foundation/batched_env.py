@@ -563,6 +563,20 @@ class BatchedFoundationEnv:
     def action_buffers(self):
         return self._stepper.buf["actions_agent"], self._stepper.buf["actions_planner"]
 
+    def sample_actions(self, logits_agent, logits_planner=None, *, seed, greedy=False, out=None):
+        """A policy's actions, drawn on the device into `action_buffers` (then step(env.action_buffers) consumes them).
+
+        One categorical per mask segment of every replica: the whole mask row of a single-action agent, each subspace of
+        a multi-action agent (with its own NO-OP), each planner bracket (or the single-action planner's one index), from
+        the softmax of the logits restricted to the open entries of the current masks (env.obs_tensors["mask_*"]).
+        logits_agent: [E, A, Na] laid out like mask_agent; logits_planner: [E, Np] like mask_planner, required when the
+        config has planner actions (ignored otherwise).  Contiguous float32 or bfloat16 (the same for both) on the env's
+        device, whatever obs_dtype is.  greedy=True: the masked argmax (evaluation).  The draws are a function of
+        (seed, number of earlier sample_actions calls, replica, agent, segment).  Returns (log_prob_agent [E, A, n_act],
+        log_prob_planner [E, n_act_p] or None), float32: buffers of the env reused by the next call, or the caller's
+        `out` = (log_prob_agent, log_prob_planner) tensors (e.g. a rollout slot; either may be None).  Asynchronous."""
+        return self._stepper.sample_policy(logits_agent, logits_planner, seed=seed, greedy=greedy, out=out)
+
     # ------------------------------------------------------------------ outputs
     @staticmethod
     def _named_fields(flat, layout):

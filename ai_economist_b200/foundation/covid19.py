@@ -286,6 +286,14 @@ class CovidBatchedEnv:
         """(agent actions [E, S], planner actions [E]): write in place and call step(env.action_buffers) for zero copies."""
         return self._stepper.buf["actions_agent"], self._stepper.buf["actions_planner"]
 
+    def sample_actions(self, logits_agent, logits_planner=None, *, seed, greedy=False, out=None):
+        """A policy's actions, drawn on the device into `action_buffers` from the softmax of its logits restricted to the
+        open entries of the current masks (greedy=True: the masked argmax).  logits_agent: [E, 51, 1 + stringency levels]
+        (action axis last; obs["a"]["action_mask"] is [E, 1 + levels, 51]); logits_planner: [E, 1 + subsidy levels];
+        contiguous float32 or bfloat16 on the env's device.  Returns (log_prob_agent [E, 51], log_prob_planner [E]),
+        float32: buffers of the env reused by the next call, or the caller's `out` tensors.  Asynchronous."""
+        return self._stepper.sample_policy(logits_agent, logits_planner, seed=seed, greedy=greedy, out=out)
+
     def _build_views(self):
         b = self._stepper.buf
         S = self.n_agents

@@ -12,7 +12,75 @@ def bf16_bits_to_float32(a):
     return (np.asarray(a).astype(np.uint32) << 16).view(np.float32)
 
 
-class BatchStepper:
+def buf_kind_numpy(buf):
+    """"f32" / "bf16" for a C-contiguous float32 / uint16 (raw bfloat16 bits) numpy array, else None."""
+    if isinstance(buf, np.ndarray) and buf.flags["C_CONTIGUOUS"]:
+        return {np.dtype(np.float32): "f32", np.dtype(np.uint16): "bf16"}.get(buf.dtype)
+    return None
+
+
+def buf_kind_torch(torch, device, buf):
+    """"f32" / "bf16" for a contiguous float32 / bfloat16 tensor on `device`, else None."""
+    if isinstance(buf, torch.Tensor) and buf.device == device and buf.is_contiguous():
+        return {torch.float32: "f32", torch.bfloat16: "bf16"}.get(buf.dtype)
+    return None
+
+
+class PolicySampler:
+    """sample_policy() of a stepper: a policy's actions drawn on the device from its logits under the env's current
+    masks (aie_sample_policy / aie_covid_sample_policy).  The stepper provides _policy_fn (the ABI entry point),
+    _policy_shapes() -> (agent logits, planner logits or None, agent log-probs, planner log-probs or None) and
+    _buf_kind(buf) ("f32" | "bf16" | None: not a contiguous float buffer of this backend's device)."""
+
+    def sample_policy(self, logits_agent, logits_planner=None, seed=0, greedy=False, out=None):
+        """Overwrite the action buffers with one draw per mask segment (greedy=True: the masked argmax) and return
+        (log_prob_agent, log_prob_planner): float32 buffers shaped like the action buffers (log_prob_planner is None
+        without planner actions).  They are the stepper's own, reused by every call, unless `out` = (log_prob_agent,
+        log_prob_planner) names the caller's (either may be None).  Asynchronous on the stream.  Logits: contiguous
+        float32 or bfloat16 (raw uint16 bits on numpy backends), both of the same dtype, on the stepper's device;
+        anything else is a ValueError before the library is called."""
+        sa, sp, sla, slp = self._policy_shapes()
+        kind = self._buf_kind(logits_agent)
+        if kind is None or tuple(logits_agent.shape) != sa:
+            raise ValueError("logits_agent must be a contiguous float32 or bfloat16 %s tensor on the env's device" % (sa,))
+        if sp is not None:
+            if logits_planner is None:
+                raise ValueError("logits_planner is required: this config has planner actions")
+            if self._buf_kind(logits_planner) != kind or tuple(logits_planner.shape) != sp:
+                raise ValueError("logits_planner must be a contiguous %s tensor of shape %s on the env's device (the dtype "
+                                 "of logits_agent)" % ("float32" if kind == "f32" else "bfloat16", sp))
+        lp_a, lp_p = (None, None) if out is None else out
+        if getattr(self, "_policy_lp", None) is None:
+            self._policy_lp = {}
+        if lp_a is None:
+            lp_a = self._policy_lp.get("a")
+            if lp_a is None:
+                lp_a = self._policy_lp["a"] = self._alloc(sla, "f32")
+        elif self._buf_kind(lp_a) != "f32" or tuple(lp_a.shape) != sla:
+            raise ValueError("out[0] must be a contiguous float32 %s tensor on the env's device" % (sla,))
+        if slp is None:
+            lp_p = None
+        elif lp_p is None:
+            lp_p = self._policy_lp.get("p")
+            if lp_p is None:
+                lp_p = self._policy_lp["p"] = self._alloc(slp, "f32")
+        elif self._buf_kind(lp_p) != "f32" or tuple(lp_p.shape) != slp:
+            raise ValueError("out[1] must be a contiguous float32 %s tensor on the env's device" % (slp,))
+        p = _abi.AiePolicyLogits()
+        p.agent = self._ptr(logits_agent)
+        p.planner = self._ptr(logits_planner) if sp is not None else None
+        p.logits_dtype = _abi.OBS_BF16 if kind == "bf16" else _abi.OBS_F32
+        p.greedy = 1 if greedy else 0
+        p.log_prob_agent = self._ptr(lp_a)
+        p.log_prob_planner = self._ptr(lp_p) if lp_p is not None else None
+        self._check(self._policy_fn(self._h, C.byref(p), C.c_uint64(int(seed)), self._stream()))
+        return lp_a, lp_p
+
+    def _buf_kind(self, buf):
+        return buf_kind_numpy(buf)
+
+
+class BatchStepper(PolicySampler):
     """Backend-agnostic part (buffer bookkeeping + ABI calls).  Subclasses supply allocation.
 
     Reference counterpart: FoundationEnvWrapper (ai_economist/foundation/env_wrapper.py:84-418), which owns
@@ -270,6 +338,16 @@ class BatchStepper:
         buffers inside the observation pass (no sampler launch per step); 0 turns it off (aie_set_fused_policy)."""
         self._check(self.lib.aie_set_fused_policy(self._h, C.c_uint64(int(seed)), self._stream()))
 
+    @property
+    def _policy_fn(self):
+        return self.lib.aie_sample_policy
+
+    def _policy_shapes(self):
+        d, E, A = self.dims, self.n_envs, self.spec["n_agents"]
+        has_p = d.n_act_planner > 0
+        return ((E, A, d.mask_agent), (E, d.mask_planner) if has_p else None, (E, A, d.n_act_agent),
+                (E, d.n_act_planner) if has_p else None)
+
     def step_host(self, actions_agent, actions_planner, out_ptrs, compact=False, n_threads=0):
         """End-to-end step with HOST buffers (aie_step_host).  out_ptrs: dict name -> host pointer / None.
         compact=True: same bytes in the host tensors, bit- / byte-packed over PCIe (aie_step_host_compact)."""
@@ -399,6 +477,9 @@ class CudaStepper(BatchStepper):
         t = self.torch
         return (isinstance(buf, t.Tensor) and buf.dtype == like.dtype and buf.shape == like.shape and buf.is_contiguous()
                 and buf.device == self.device)
+
+    def _buf_kind(self, buf):
+        return buf_kind_torch(self.torch, self.device, buf)
 
     def _ptr(self, buf):
         return C.c_void_p(buf.data_ptr())

@@ -393,6 +393,35 @@ int aie_sample_random_actions(aie_env *env, uint64_t seed, void *stream);
  * and then only aie_step. */
 int aie_set_fused_policy(aie_env *env, uint64_t seed, void *stream);
 
+/* A policy's logits, laid out like the masks with the action axis last, and where the log-probabilities go. */
+typedef struct aie_policy_logits {
+    const void *agent;        /* DEVICE [E, A, Na] (the mask_agent layout, each multi-action subspace with its own NO-OP) */
+    const void *planner;      /* DEVICE [E, Np] (the mask_planner layout), or NULL when the config has no planner actions */
+    int32_t logits_dtype;     /* AIE_OBS_F32 | AIE_OBS_BF16 (independent of the config's obs_dtype) */
+    int32_t greedy;           /* 0: draw from the softmax; 1: the open entry with the largest logit (lowest index on ties) */
+    float *log_prob_agent;    /* DEVICE [E, A, n_act_a] or NULL */
+    float *log_prob_planner;  /* DEVICE [E, n_act_p] or NULL */
+} aie_policy_logits;
+
+/* ABI 5.  A policy's actions on the device: for every env, agent (every subspace in multi-action mode) and planner
+ * bracket (or the single-action planner's one index), one draw from the softmax of the segment's logits restricted to
+ * the open entries of the CURRENT mask buffers (what the latest reset / step / observe wrote), into the bound action
+ * buffers (whatever was there is overwritten, the fused random policy's draw included); the log-probability of each
+ * action into the optional log_prob tensors.  One launch, asynchronous on `stream`.
+ *   Stream: s = host_mix64(seed) ^ host_mix64(n), n = 1, 2, .. counting this env's aie_sample_policy calls (its own
+ *   counter: aie_sample_random_actions does not move it); env key k = mix64(s ^ mix64(env)) (mix64: the splitmix64
+ *   finaliser); segment key k + 0x100 * agent (single-action agents), k + 0x100 * agent + subspace + 1 (multi-action),
+ *   k + 0x10000 + bracket (planner brackets; bracket 0 for the single-action planner); u = (mix64(segment key) >> 11) * 2^-53.
+ *   Draw (float64): m = the largest open logit, w_j = exp((double)l_j - m) for open j (0 for closed), Z = sum w_j; the
+ *   action is the smallest j with w_j > 0 and u * Z < w_0 + .. + w_j, else (rounding) the last j with w_j > 0.
+ *   greedy = 1: the first open j with l_j == m.  Log-probability: (float)(((double)l_a - m) - log(Z)).
+ *   A segment with no open entry: action 0, log-probability 0.  An open logit that is NaN or +inf, or no finite open
+ *   logit: the first open entry, log-probability NaN.  Open entries at -inf are never drawn.
+ * AIE_EINVAL for a NULL p or agent logits, missing planner logits when the config has planner actions, an unknown
+ * logits_dtype, greedy not 0 or 1, or a pointer not aligned to its element size; AIE_ESTATE before buffers are bound
+ * and state is loaded. */
+int aie_sample_policy(aie_env *env, const aie_policy_logits *p, uint64_t seed, void *stream);
+
 /* End-to-end variant with HOST buffers: copies the actions host->device, steps, copies every non-NULL
  * output device->host, and synchronises the stream.  Buffers should be pinned for full PCIe rate. */
 int aie_step_host(aie_env *env, const int32_t *actions_agent_host, const int32_t *actions_planner_host,
@@ -524,6 +553,12 @@ int aie_covid_reset(aie_covid_env *env, void *stream);
 int aie_covid_step(aie_covid_env *env, void *stream);
 /* Random policy on the device (uniform over the unmasked actions of the current masks); see aie_sample_random_actions. */
 int aie_covid_sample_random_actions(aie_covid_env *env, uint64_t seed, void *stream);
+/* A policy's actions on the device (the contract of aie_sample_policy): agent logits [E, S, 1 + levels] (action axis
+ * last; the mask they are read against is mask_agent [E, 1 + levels, S]), planner logits [E, 1 + subsidy levels]
+ * (required); log-probabilities [E, S] and [E].  Keys as the random policy's: env key k = cv_mix64(s ^ cv_mix64(env))
+ * with s = host_mix64(seed) ^ host_mix64(n), n counting this env's aie_covid_sample_policy calls; state a draws with
+ * k + 0x100 * a, the planner with k ^ 0xabcdef.  AIE_EINVAL also when 1 + subsidy levels > 160. */
+int aie_covid_sample_policy(aie_covid_env *env, const aie_policy_logits *p, uint64_t seed, void *stream);
 int64_t aie_covid_launch_count(const aie_covid_env *env);
 
 const char *aie_last_error(void);
