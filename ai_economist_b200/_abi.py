@@ -126,6 +126,15 @@ class AiePolicyLogits(C.Structure):
                 ("log_prob_agent", C.c_void_p), ("log_prob_planner", C.c_void_p)]
 
 
+class AiePolicyEval(C.Structure):
+    _fields_ = ([(n, C.c_void_p) for n in ["logits_agent", "logits_planner", "mask_agent", "mask_planner",
+                                           "actions_agent", "actions_planner"]]
+                + [("logits_dtype", C.c_int32), ("mask_dtype", C.c_int32)]
+                + [(n, C.c_void_p) for n in ["log_prob_agent", "log_prob_planner", "entropy_agent", "entropy_planner",
+                                             "grad_log_prob_agent", "grad_log_prob_planner", "grad_entropy_agent",
+                                             "grad_entropy_planner", "grad_logits_agent", "grad_logits_planner"]])
+
+
 class AieCovidConfig(C.Structure):
     _fields_ = ([(n, C.c_int32) for n in [
         "abi_version", "n_states", "episode_length", "num_stringency_levels", "action_cooldown_period",
@@ -191,6 +200,10 @@ def load_library(path=None):
     L.aie_sample_policy.restype = C.c_int
     L.aie_covid_sample_policy.argtypes = [P, C.POINTER(AiePolicyLogits), C.c_uint64, P]
     L.aie_covid_sample_policy.restype = C.c_int
+    for fn in ["aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_covid_evaluate_policy",
+               "aie_covid_evaluate_policy_backward"]:
+        getattr(L, fn).argtypes = [P, C.POINTER(AiePolicyEval), C.c_int64, P]
+        getattr(L, fn).restype = C.c_int
     L.aie_step_host.argtypes = [P, P, P, C.POINTER(AieHostOut), P]
     L.aie_step_host_compact.argtypes = [P, P, P, C.POINTER(AieHostOut), C.c_int32, P]
     L.aie_step_host_compact.restype = C.c_int
@@ -229,10 +242,11 @@ def load_library(path=None):
 
 EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field", "aie_get_flat_layout", "aie_bind_buffers",
                     "aie_load_state", "aie_reset_envs", "aie_step", "aie_step_dynamics", "aie_observe", "aie_observe_final", "aie_sample_random_actions",
-                    "aie_set_fused_policy", "aie_sample_policy", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
+                    "aie_set_fused_policy", "aie_sample_policy", "aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
                     "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
-                    "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_launch_count"]
+                    "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
+                    "aie_covid_evaluate_policy_backward", "aie_covid_launch_count"]
 
 
 def obs_dtype_name(obs_dtype):

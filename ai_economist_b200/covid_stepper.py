@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from .stepper import PolicySampler, buf_kind_torch
+from .stepper import PolicySampler, buf_kind_torch, is_i32_torch
 
 F32, I32 = np.float32, np.int32
 
@@ -141,6 +141,14 @@ class CovidStepperBase(PolicySampler):
         E, S = self.n_envs, self.p["n_states"]
         return ((E, S, 1 + self.p["num_stringency_levels"]), (E, 1 + self.p["num_subsidy_levels"]), (E, S), (E,))
 
+    @property
+    def _eval_fns(self):
+        return self.lib.aie_covid_evaluate_policy, self.lib.aie_covid_evaluate_policy_backward
+
+    def _mask_rows(self):   # evaluate_policy: the agent mask is [*B, 1 + levels, S], transposed against the logits
+        S, L = self.p["n_states"], self.p["num_stringency_levels"]
+        return (1 + L, S), (1 + self.p["num_subsidy_levels"],)
+
     def launch_count(self):
         return int(self.lib.aie_covid_launch_count(self._h))
 
@@ -181,6 +189,13 @@ class CudaCovidStepper(CovidStepperBase):
 
     def _buf_kind(self, buf):
         return buf_kind_torch(self.torch, self.device, buf)
+
+    def _is_i32(self, buf):
+        return is_i32_torch(self.torch, self.device, buf)
+
+    def _eval_out(self, shape, kind):
+        t = self.torch
+        return t.empty(shape, dtype={"f32": t.float32, "bf16": t.bfloat16}[kind], device=self.device)
 
     def _ptr(self, buf):
         return C.c_void_p(buf.data_ptr())

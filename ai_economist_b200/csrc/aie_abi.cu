@@ -16,6 +16,12 @@
 //                          from its logits under the current masks (aie_sample_policy), with their log-probabilities;
 //                          *_bf16 reads bfloat16 masks, and each is instantiated for float32 and bfloat16 logits.
 //   aie_covid_sample_policy_kernel  one warp per (env, state | planner): the same for the COVID-19 scenario.
+//   aie_evaluate_policy_kernel, aie_evaluate_policy_backward_kernel  one warp per row of stored actions, or per (row,
+//                          unit) for many agent segments: log-probabilities and entropies of stored actions under
+//                          stored masks (aie_evaluate_policy), and their gradient with respect to the logits
+//                          (aie_evaluate_policy_backward); instantiated for float32 / bfloat16 masks and logits.
+//   aie_covid_evaluate_policy_kernel, aie_covid_evaluate_policy_backward_kernel  one warp per (row, state | planner):
+//                          the same for the COVID-19 scenario.
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
 // aie_config::obs_dtype == AIE_OBS_BF16); the launchers pick one from the config, with the same launch shape.
 #include <cuda_runtime.h>
@@ -101,6 +107,9 @@ int covid_launch_reset(aie_covid_env *, void *stream);
 int covid_launch_step(aie_covid_env *, void *stream);
 int covid_launch_sample(aie_covid_env *, uint64_t key, void *stream);
 int covid_launch_policy(aie_covid_env *, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream);
+int launch_policy_eval(aie_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows, void *stream);
+int covid_launch_policy_eval(aie_covid_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows,
+                             void *stream);
 }  // namespace be
 }  // namespace aie
 
@@ -569,6 +578,27 @@ __global__ void __launch_bounds__(256, 2) aie_sample_policy_bf16_kernel(const __
     policy_kernel_body<EXT, bf16_t, LT>(c, b, p, seed, per_unit);
 }
 
+// Evaluation of stored actions (aie_evaluate_policy, aie_evaluate_policy_backward): per_unit 0: one warp per row,
+// 1: one warp per (row, unit), units = A + n_act_p; MT: the masks' element type, LT: the logits' and gradients'.
+template <bool BWD, typename MT, typename LT>
+__device__ __forceinline__ void policy_eval_kernel_body(const DevCfg &c, const PolicyEvalBufs &p, long long n_rows, int per_unit) {
+    const long long wid = (long long)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
+    const int units = per_unit ? c.A + c.n_act_p : 1;
+    const long long r = wid / units;
+    if (r >= n_rows) return;
+    policy_eval_row<BWD, MT, LT>(c, p, r, per_unit ? (int)(wid - r * units) : -1, threadIdx.x & 31);
+}
+template <typename MT, typename LT>
+__global__ void __launch_bounds__(256) aie_evaluate_policy_kernel(const __grid_constant__ DevCfg c, const PolicyEvalBufs p,
+                                                                  long long n_rows, int per_unit) {
+    policy_eval_kernel_body<false, MT, LT>(c, p, n_rows, per_unit);
+}
+template <typename MT, typename LT>
+__global__ void __launch_bounds__(256) aie_evaluate_policy_backward_kernel(const __grid_constant__ DevCfg c,
+                                                                           const PolicyEvalBufs p, long long n_rows, int per_unit) {
+    policy_eval_kernel_body<true, MT, LT>(c, p, n_rows, per_unit);
+}
+
 // ---------------------------------------------------------------------------------------------------------
 namespace be {
 
@@ -935,6 +965,33 @@ int launch_policy(aie_env *env, const PolicyBufs &p, int lt_bf16, uint64_t sd, v
     return AIE_OK;
 }
 
+// Row count times units over eight warps per CTA must fit the grid's x dimension.
+static int eval_grid(long long n_rows, int units, unsigned &grid) {
+    const long long ctas = (n_rows * units + 7) / 8;
+    if (ctas > 0x7fffffffLL) return fail(AIE_EINVAL, "aie_evaluate_policy: too many rows for one launch");
+    grid = (unsigned)ctas;
+    return AIE_OK;
+}
+int launch_policy_eval(aie_env *env, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows, void *stream) {
+    const DevCfg &c = env->cfg;
+    int per_unit = (c.A * c.n_act_a >= POLICY_PER_UNIT_MIN) ? 1 : 0;
+    if (const char *v = getenv("AIE_POLICY_PER_UNIT")) per_unit = atoi(v) ? 1 : 0;   // timing aid (tools/time_evaluate_actions.py)
+    unsigned grid;
+    if (eval_grid(n_rows, per_unit ? c.A + c.n_act_p : 1, grid) != AIE_OK) return AIE_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+#define AIE_EVAL_LAUNCH(MT, LT)                                                                              \
+    (bwd ? aie_evaluate_policy_backward_kernel<MT, LT><<<grid, 256, 0, st>>>(c, p, n_rows, per_unit)          \
+         : aie_evaluate_policy_kernel<MT, LT><<<grid, 256, 0, st>>>(c, p, n_rows, per_unit))
+    if (mt_bf16) {
+        if (lt_bf16) AIE_EVAL_LAUNCH(bf16_t, bf16_t);
+        else AIE_EVAL_LAUNCH(bf16_t, float);
+    } else if (lt_bf16) AIE_EVAL_LAUNCH(float, bf16_t);
+    else AIE_EVAL_LAUNCH(float, float);
+#undef AIE_EVAL_LAUNCH
+    AIE_CUDA(cudaGetLastError(), bwd ? "aie_evaluate_policy_backward_kernel launch" : "aie_evaluate_policy_kernel launch");
+    return AIE_OK;
+}
+
 }  // namespace be
 
 // ---------------------------------------------------------------------------------------------------------
@@ -960,6 +1017,26 @@ __global__ void __launch_bounds__(256) aie_covid_sample_policy_kernel(const __gr
     const int env = (int)(wid / units), u = (int)(wid - (long long)env * units);
     if (env >= c.n_envs) return;
     covid_policy_unit<LT>(c, env, b, p, cv_mix64(sd ^ cv_mix64((uint64_t)env)), u, threadIdx.x & 31);
+}
+
+// Evaluation of stored actions (aie_covid_evaluate_policy, *_backward): one warp per (row, unit), units = S + 1.
+template <bool BWD, typename MT, typename LT>
+__device__ __forceinline__ void covid_policy_eval_body(const CovidCfg &c, const PolicyEvalBufs &p, long long n_rows) {
+    const long long wid = (long long)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
+    const int units = c.S + 1;
+    const long long r = wid / units;
+    if (r >= n_rows) return;
+    covid_policy_eval_unit<BWD, MT, LT>(c, p, r, (int)(wid - r * units), threadIdx.x & 31);
+}
+template <typename MT, typename LT>
+__global__ void __launch_bounds__(256) aie_covid_evaluate_policy_kernel(const __grid_constant__ CovidCfg c,
+                                                                        const PolicyEvalBufs p, long long n_rows) {
+    covid_policy_eval_body<false, MT, LT>(c, p, n_rows);
+}
+template <typename MT, typename LT>
+__global__ void __launch_bounds__(256) aie_covid_evaluate_policy_backward_kernel(const __grid_constant__ CovidCfg c,
+                                                                                 const PolicyEvalBufs p, long long n_rows) {
+    covid_policy_eval_body<true, MT, LT>(c, p, n_rows);
 }
 
 namespace be {
@@ -994,6 +1071,24 @@ int covid_launch_policy(aie_covid_env *env, const PolicyBufs &p, int lt_bf16, ui
     else aie_covid_sample_policy_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, p, sd);
     AIE_CUDA(cudaGetLastError(), "aie_covid_sample_policy_kernel launch");
     env->launches++;
+    return AIE_OK;
+}
+int covid_launch_policy_eval(aie_covid_env *env, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd,
+                             long long n_rows, void *stream) {
+    unsigned grid;
+    if (eval_grid(n_rows, env->cfg.S + 1, grid) != AIE_OK) return AIE_EINVAL;
+    const CovidCfg &c = env->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+#define AIE_EVAL_LAUNCH(MT, LT)                                                                              \
+    (bwd ? aie_covid_evaluate_policy_backward_kernel<MT, LT><<<grid, 256, 0, st>>>(c, p, n_rows)              \
+         : aie_covid_evaluate_policy_kernel<MT, LT><<<grid, 256, 0, st>>>(c, p, n_rows))
+    if (mt_bf16) {
+        if (lt_bf16) AIE_EVAL_LAUNCH(bf16_t, bf16_t);
+        else AIE_EVAL_LAUNCH(bf16_t, float);
+    } else if (lt_bf16) AIE_EVAL_LAUNCH(float, bf16_t);
+    else AIE_EVAL_LAUNCH(float, float);
+#undef AIE_EVAL_LAUNCH
+    AIE_CUDA(cudaGetLastError(), bwd ? "aie_covid_evaluate_policy_backward_kernel launch" : "aie_covid_evaluate_policy_kernel launch");
     return AIE_OK;
 }
 int covid_launch_step(aie_covid_env *env, void *stream) {

@@ -1636,82 +1636,46 @@ AIE_DEV float logit_value(bf16_t v) {
 }
 AIE_DEV double policy_uniform(uint64_t key) { return (double)(mix64(key) >> 11) * 0x1.0p-53; }
 
-// One segment: mask[j * ms] (ms: element stride of the mask; 1 except for the COVID agents' [levels][S] masks) and
-// logit[j], j < n <= MAX_MASK.  Returns the action on every lane and writes the log-probability to *lp on every lane.
-// Device: one warp, entry j on lane j % 32 of chunk j / 32 (five chunks); max and prefix by shuffles, crossing by ballot.
-template <typename MT, typename LT>
-AIE_DEV int policy_segment_warp(const MT *mask, int ms, const LT *logit, int n, uint64_t key, int greedy, int lane, float *lp) {
+// The open entries, m and Z of one segment: mask[j * ms] (ms: element stride of the mask; 1 except for the COVID
+// agents' [levels][S] masks) and logit[j], j < n <= MAX_MASK.  Shared by the sampler (policy_segment_warp) and the
+// evaluation (policy_segment_eval), so both sum Z in one order: on the device a float64 inclusive warp scan per chunk of
+// 32 entries (entry j on lane j % 32 of chunk j / 32) with the chunks' totals added in turn, in the host build a serial
+// sum.  Two steps, so that a caller leaves on the edge cases before the scan: policy_segment_open returns 0: no open
+// entry; 1: an open logit is NaN or +inf, or no open logit is finite; 2: policy_segment_z then sets mx and Z.
+struct PolicySeg {
+    float mx;          // the largest open logit (m = (double)mx)
+    double Z;          // sum over open j of exp((double)l_j - m)
 #if AIE_ON_DEVICE
-    float lv[5];
-    uint32_t om[5], bad = 0, fin = 0, any = 0;
+    float lv[5];       // this lane's entry of each chunk: its logit when open, else -inf
+    uint32_t om[5];    // open entries, one ballot per chunk
+    double w[5];       // this lane's w of each chunk (chunks past n: unset)
+    double cum[5];     // inclusive prefix of w over the segment, this lane's entry of each chunk (chunks past n: 0)
+    uint32_t pos[5];   // entries with w > 0
+#else
+    int first;         // the first open entry
+#endif
+};
+template <typename MT, typename LT>
+AIE_DEV int policy_segment_open(const MT *mask, int ms, const LT *logit, int n, int lane, PolicySeg &s) {
+#if AIE_ON_DEVICE
+    uint32_t bad = 0, fin = 0, any = 0;
     float mx = -INFINITY;
 #pragma unroll
     for (int ch = 0; ch < 5; ch++) {
         const int j = ch * NL + lane;
         const bool o = j < n && mask_open(mask[(size_t)j * ms]);
         const float v = o ? logit_value(logit[j]) : -INFINITY;
-        lv[ch] = v;
-        om[ch] = wballot(o);
-        any |= om[ch];
+        s.lv[ch] = v;
+        s.om[ch] = wballot(o);
+        any |= s.om[ch];
         bad |= wballot(o && !(v < INFINITY));          // NaN or +inf
         fin |= wballot(o && v > -INFINITY && v < INFINITY);
         mx = fmaxf(mx, v);
     }
-    if (!any) { *lp = 0.0f; return 0; }
-    if (bad || !fin) {
-        *lp = __int_as_float(0x7fc00000);
-#pragma unroll
-        for (int ch = 0; ch < 5; ch++)
-            if (om[ch]) return ch * NL + first_lane(om[ch]);
-        return 0;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    const double m = (double)mx;
-    double cum[5];
-    uint32_t pos[5];
-    double carry = 0.0;
-#pragma unroll
-    for (int ch = 0; ch < 5; ch++) {
-        cum[ch] = 0.0; pos[ch] = 0u;
-        if (ch * NL < n) {   // warp-uniform
-            const double w = ((om[ch] >> lane) & 1u) ? exp((double)lv[ch] - m) : 0.0;
-            pos[ch] = wballot(w > 0.0);
-            double s = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const double t = __shfl_up_sync(0xffffffffu, s, o);
-                if (lane >= o) s += t;
-            }
-            cum[ch] = carry + s;
-            carry = __shfl_sync(0xffffffffu, cum[ch], 31);
-        }
-    }
-    const double Z = carry;
-    int a = -1;
-    if (greedy) {
-#pragma unroll
-        for (int ch = 0; ch < 5; ch++) {
-            const uint32_t hit = wballot(((om[ch] >> lane) & 1u) && lv[ch] == mx);
-            if (a < 0 && hit) a = ch * NL + first_lane(hit);
-        }
-    } else {
-        const double t = policy_uniform(key) * Z;
-#pragma unroll
-        for (int ch = 0; ch < 5; ch++) {
-            const uint32_t hit = wballot(((pos[ch] >> lane) & 1u) && t < cum[ch]);
-            if (a < 0 && hit) a = ch * NL + first_lane(hit);
-        }
-        if (a < 0) {
-#pragma unroll
-            for (int ch = 0; ch < 5; ch++)
-                if (pos[ch]) a = ch * NL + 31 - __clz(pos[ch]);
-        }
-    }
-    const double la = greedy ? m : (double)logit_value(logit[a]);
-    *lp = (float)((la - m) - log(Z));
-    return a;
+    s.mx = mx;   // this lane's part (policy_segment_z reduces it)
+    return !any ? 0 : (bad || !fin) ? 1 : 2;
 #else
+    (void)lane;
     int first = -1;
     bool bad = false, fin = false;
     float mx = -INFINITY;
@@ -1722,12 +1686,95 @@ AIE_DEV int policy_segment_warp(const MT *mask, int ms, const LT *logit, int n, 
         if (!(v < INFINITY)) bad = true;
         else if (v > -INFINITY) { fin = true; mx = v > mx ? v : mx; }
     }
-    if (first < 0) { *lp = 0.0f; return 0; }
-    if (bad || !fin) { *lp = NAN; return first; }
+    s.first = first;
+    s.mx = mx;
+    return first < 0 ? 0 : (bad || !fin) ? 1 : 2;
+#endif
+}
+template <typename MT, typename LT>
+AIE_DEV void policy_segment_z(const MT *mask, int ms, const LT *logit, int n, int lane, PolicySeg &s) {
+#if AIE_ON_DEVICE
+    (void)mask; (void)ms; (void)logit;
+    float mx = s.mx;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    s.mx = mx;
     const double m = (double)mx;
+    double carry = 0.0;
+#pragma unroll
+    for (int ch = 0; ch < 5; ch++) {
+        s.cum[ch] = 0.0; s.pos[ch] = 0u;
+        if (ch * NL < n) {   // warp-uniform
+            const double w = ((s.om[ch] >> lane) & 1u) ? exp((double)s.lv[ch] - m) : 0.0;
+            s.w[ch] = w;
+            s.pos[ch] = wballot(w > 0.0);
+            double t = w;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const double u = __shfl_up_sync(0xffffffffu, t, o);
+                if (lane >= o) t += u;
+            }
+            s.cum[ch] = carry + t;
+            carry = __shfl_sync(0xffffffffu, s.cum[ch], 31);
+        }
+    }
+    s.Z = carry;
+#else
+    (void)lane;
+    const double m = (double)s.mx;
     double Z = 0.0;
     for (int j = 0; j < n; j++)
         if (mask_open(mask[(size_t)j * ms])) Z += exp((double)logit_value(logit[j]) - m);
+    s.Z = Z;
+#endif
+}
+
+// One segment of the sampler (the layout of policy_segment_open).  Returns the action on every lane and writes the
+// log-probability to *lp on every lane.  Device: one warp; the crossing of u * Z is found by ballots over the prefix.
+template <typename MT, typename LT>
+AIE_DEV int policy_segment_warp(const MT *mask, int ms, const LT *logit, int n, uint64_t key, int greedy, int lane, float *lp) {
+    PolicySeg s;
+    const int st = policy_segment_open(mask, ms, logit, n, lane, s);
+    if (st == 0) { *lp = 0.0f; return 0; }
+#if AIE_ON_DEVICE
+    if (st == 1) {
+        *lp = __int_as_float(0x7fc00000);
+#pragma unroll
+        for (int ch = 0; ch < 5; ch++)
+            if (s.om[ch]) return ch * NL + first_lane(s.om[ch]);
+        return 0;
+    }
+    policy_segment_z(mask, ms, logit, n, lane, s);
+    const float mx = s.mx;
+    const double m = (double)mx, Z = s.Z;
+    int a = -1;
+    if (greedy) {
+#pragma unroll
+        for (int ch = 0; ch < 5; ch++) {
+            const uint32_t hit = wballot(((s.om[ch] >> lane) & 1u) && s.lv[ch] == mx);
+            if (a < 0 && hit) a = ch * NL + first_lane(hit);
+        }
+    } else {
+        const double t = policy_uniform(key) * Z;
+#pragma unroll
+        for (int ch = 0; ch < 5; ch++) {
+            const uint32_t hit = wballot(((s.pos[ch] >> lane) & 1u) && t < s.cum[ch]);
+            if (a < 0 && hit) a = ch * NL + first_lane(hit);
+        }
+        if (a < 0) {
+#pragma unroll
+            for (int ch = 0; ch < 5; ch++)
+                if (s.pos[ch]) a = ch * NL + 31 - __clz(s.pos[ch]);
+        }
+    }
+    const double la = greedy ? m : (double)logit_value(logit[a]);
+    *lp = (float)((la - m) - log(Z));
+    return a;
+#else
+    if (st == 1) { *lp = NAN; return s.first; }
+    policy_segment_z(mask, ms, logit, n, lane, s);
+    const float mx = s.mx;
+    const double m = (double)mx, Z = s.Z;
     int a = -1;
     if (greedy) {
         for (int j = 0; j < n && a < 0; j++)
@@ -1803,6 +1850,161 @@ AIE_DEV void policy_actions_env(const DevCfg &c, const DevBufs &b, const PolicyB
     if (u >= 0) { policy_actions_unit<EXT>(c, am, pm, al, pl, aa, ap, la, lq, key, p.greedy, u, lane); return; }
     const int units = c.A + (c.planner_acts ? c.B : 0);
     for (int v = 0; v < units; v++) policy_actions_unit<EXT>(c, am, pm, al, pl, aa, ap, la, lq, key, p.greedy, v, lane);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Evaluation of stored actions (aie_evaluate_policy, aie_evaluate_policy_backward): per mask segment, the
+// log-probability of the stored action a and the entropy of the softmax of the logits restricted to the open entries,
+// and the gradient of g_lp * lp + g_H * H with respect to the logits.  m and Z are policy_segment_open / _z's, the
+// sampler's own, so lp is bit for bit what the sampler returned for (logits, masks, a).  In float64, rounded once:
+//   lp = (float)(((double)l_a - m) - log Z),  H = (float)(log Z - sum_j p_j (l_j - m)),  p_j = w_j / Z;
+//   gradient of open j: g_lp ([j = a] - p_j) - g_H p_j ((l_j - m - log Z) + H), closed j: 0.
+// No open entry: lp = H = 0, gradient 0.  An open logit NaN or +inf, or none finite: lp = H = NaN, the open entries'
+// gradient NaN.  a closed or outside [0, n): lp = NaN, the open entries' gradient NaN, H as usual (a is read, never
+// the mask or logit outside the segment).  An open entry with w_j = 0 (at -inf) has p_j = 0: no entropy term.
+// The backward recomputes m and Z from the logits; nothing of the forward is stored.
+// ------------------------------------------------------------------------------------------------
+// round-to-nearest-even bfloat16 bits of a float64 value without double rounding: to float32 rounded to odd (toward
+// zero, the last bit set when inexact), then to nearest even (NaN -> a quiet NaN)
+AIE_DEV uint16_t bf16_from_double(double x) {
+    if (x != x) return 0x7FC0u;
+    const float f = (float)x;
+    uint32_t u;
+#if AIE_ON_DEVICE
+    u = __float_as_uint(f);
+#else
+    memcpy(&u, &f, 4);
+#endif
+    if ((double)f != x) {
+        if (fabs((double)f) > fabs(x)) u -= 1u;   // one step toward zero (from +-inf on overflow: +-FLT_MAX)
+        u |= 1u;
+    }
+    return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+}
+AIE_DEV void put_grad(float *p, double g) { *p = (float)g; }
+AIE_DEV void put_grad(bf16_t *p, double g) { p->bits = bf16_from_double(g); }
+
+// One segment (the layout of policy_segment_open), the stored action at *act.  Forward (BWD false): lp and H to *lp,
+// *h from lane 0.  Backward: g_lp = *glp and g_H = *gh (null: 0), the gradient of entries j < n to grad[j].
+template <bool BWD, typename MT, typename LT>
+AIE_DEV void policy_segment_eval(const MT *mask, int ms, const LT *logit, int n, const int32_t *act, const float *glp,
+                                 const float *gh, float *lp, float *h, LT *grad, int lane) {
+    PolicySeg s;
+    const int st = policy_segment_open(mask, ms, logit, n, lane, s);
+    if (st == 2) policy_segment_z(mask, ms, logit, n, lane, s);
+    const int a = *act;
+    const bool ok = a >= 0 && a < n && mask_open(mask[(size_t)a * ms]);
+    double m = 0.0, Z = 1.0, lz = 0.0, H = 0.0;
+    if (st == 2) {
+        m = (double)s.mx;
+        Z = s.Z;
+        lz = log(Z);
+        double e = 0.0;   // sum over open j of w_j (l_j - m)
+#if AIE_ON_DEVICE
+#pragma unroll
+        for (int ch = 0; ch < 5; ch++)
+            if (ch * NL < n && s.w[ch] > 0.0) e += s.w[ch] * ((double)s.lv[ch] - m);
+        e = wsum(e);
+#else
+        for (int j = 0; j < n; j++) {
+            if (!mask_open(mask[(size_t)j * ms])) continue;
+            const double d = (double)logit_value(logit[j]) - m, w = exp(d);
+            if (w > 0.0) e += w * d;
+        }
+#endif
+        H = lz - e / Z;
+    }
+    if (!BWD) {
+        if (lane == 0) {
+            if (st == 2) {
+                *lp = ok ? (float)(((double)logit_value(logit[a]) - m) - lz) : NAN;
+                *h = (float)H;
+            } else {
+                *lp = *h = st ? NAN : 0.0f;
+            }
+        }
+        return;
+    }
+    const double g_lp = glp ? (double)*glp : 0.0, g_h = gh ? (double)*gh : 0.0;
+    const bool nan_open = st == 1 || (st == 2 && !ok);
+#if AIE_ON_DEVICE
+#pragma unroll
+    for (int ch = 0; ch < 5; ch++) {
+        const int j = ch * NL + lane;
+        if (j < n) {
+            double g = 0.0;
+            if ((s.om[ch] >> lane) & 1u) {
+                if (nan_open) {
+                    g = NAN;
+                } else {
+                    const double p = s.w[ch] / Z;
+                    g = g_lp * ((j == a ? 1.0 : 0.0) - p);
+                    if (p > 0.0) g -= g_h * p * ((((double)s.lv[ch] - m) - lz) + H);
+                }
+            }
+            put_grad(grad + j, g);
+        }
+    }
+#else
+    for (int j = 0; j < n; j++) {
+        double g = 0.0;
+        if (mask_open(mask[(size_t)j * ms])) {
+            if (nan_open) {
+                g = NAN;
+            } else {
+                const double d = (double)logit_value(logit[j]) - m, p = exp(d) / Z;
+                g = g_lp * ((j == a ? 1.0 : 0.0) - p);
+                if (p > 0.0) g -= g_h * p * ((d - lz) + H);
+            }
+        }
+        put_grad(grad + j, g);
+    }
+#endif
+}
+
+// Where aie_evaluate_policy reads and writes (device pointers; rows of the leading batch, N of them, at r * row size)
+struct PolicyEvalBufs {
+    const void *a_logit, *p_logit;              // [N][A][Na], [N][Np] (COVID-19: [N][S][1 + levels], [N][1 + sub levels]): LT
+    const void *a_mask, *p_mask;                // the mask layouts (COVID-19 agents: [N][1 + levels][S]): MT
+    const int32_t *act_a, *act_p;               // [N][A][n_act_a], [N][n_act_p] (COVID-19: [N][S], [N])
+    float *lp_a, *lp_p, *h_a, *h_p;             // forward: log-probabilities and entropies, shaped like the actions
+    const float *glp_a, *glp_p, *gh_a, *gh_p;   // backward: their upstream gradients, or null (zero)
+    void *g_a, *g_p;                            // backward: the gradient with respect to the logits (LT, their layout)
+};
+// One segment of row r, slot k of its actions, entries at off of its logits and masks (ms: the masks' stride).
+template <bool BWD, typename MT, typename LT>
+AIE_DEV void policy_eval_slot(const MT *mask, int ms, const void *logit, int n, size_t off, const int32_t *act,
+                              const float *glp, const float *gh, float *lp, float *h, void *grad, size_t k, int lane) {
+    policy_segment_eval<BWD>(mask, ms, (const LT *)logit + off, n, act + k, BWD && glp ? glp + k : nullptr,
+                             BWD && gh ? gh + k : nullptr, BWD ? nullptr : lp + k, BWD ? nullptr : h + k,
+                             BWD ? (LT *)grad + off : nullptr, lane);
+}
+// One unit of row r: u < A is agent u (every subspace in multi-action mode), u = A + b planner slot b (a bracket, or
+// the single-action planner's one index).
+template <bool BWD, typename MT, typename LT>
+AIE_DEV void policy_eval_unit(const DevCfg &c, const PolicyEvalBufs &p, long long r, int u, int lane) {
+    if (u < c.A) {
+        const size_t row = ((size_t)r * c.A + u) * c.Na, slot = ((size_t)r * c.A + u) * c.n_act_a;
+        int off = 0;
+        for (int si = 0; si < c.n_act_a; si++) {
+            const int n = c.multi_action ? c.sub_n[si] + 1 : c.Na;
+            policy_eval_slot<BWD, MT, LT>((const MT *)p.a_mask + row + off, 1, p.a_logit, n, row + off, p.act_a, p.glp_a,
+                                          p.gh_a, p.lp_a, p.h_a, p.g_a, slot + si, lane);
+            off += n;
+        }
+    } else {
+        const int b = u - c.A, n = c.planner_single ? c.Np : 1 + c.R;
+        const size_t off = (size_t)r * c.Np + (size_t)b * n;
+        policy_eval_slot<BWD, MT, LT>((const MT *)p.p_mask + off, 1, p.p_logit, n, off, p.act_p, p.glp_p, p.gh_p, p.lp_p,
+                                      p.h_p, p.g_p, (size_t)r * c.n_act_p + b, lane);
+    }
+}
+// Row r: every unit (u < 0) or unit u only; units = A + n_act_p.
+template <bool BWD, typename MT, typename LT>
+AIE_DEV void policy_eval_row(const DevCfg &c, const PolicyEvalBufs &p, long long r, int u, int lane) {
+    if (u >= 0) { policy_eval_unit<BWD, MT, LT>(c, p, r, u, lane); return; }
+    const int units = c.A + c.n_act_p;
+    for (int v = 0; v < units; v++) policy_eval_unit<BWD, MT, LT>(c, p, r, v, lane);
 }
 
 }  // namespace aie

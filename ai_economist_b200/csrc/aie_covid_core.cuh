@@ -429,4 +429,21 @@ CV_DEV void covid_policy_unit(const CovidCfg &c, int e, const CovidBufs &b, cons
     }
 }
 
+// Evaluation of stored actions (aie_covid_evaluate_policy, policy_segment_eval in aie_core.cuh): unit u < S is state u
+// of row r, its logits [N][S][1 + levels] read against the mask column mask_a[r][.][u]; unit S is the planner, logits
+// [N][1 + sub_levels].  Actions [N][S] and [N].
+template <bool BWD, typename MT, typename LT>
+CV_DEV void covid_policy_eval_unit(const CovidCfg &c, const PolicyEvalBufs &p, long long r, int u, int lane) {
+    if (u < c.S) {
+        const int n = 1 + c.levels;
+        const size_t i = (size_t)r * c.S + u;
+        policy_eval_slot<BWD, MT, LT>((const MT *)p.a_mask + (size_t)r * n * c.S + u, c.S, p.a_logit, n, i * n, p.act_a,
+                                      p.glp_a, p.gh_a, p.lp_a, p.h_a, p.g_a, i, lane);
+    } else {
+        const int n = 1 + c.sub_levels;
+        policy_eval_slot<BWD, MT, LT>((const MT *)p.p_mask + (size_t)r * n, 1, p.p_logit, n, (size_t)r * n, p.act_p,
+                                      p.glp_p, p.gh_p, p.lp_p, p.h_p, p.g_p, (size_t)r, lane);
+    }
+}
+
 }  // namespace aie

@@ -577,6 +577,22 @@ class BatchedFoundationEnv:
         `out` = (log_prob_agent, log_prob_planner) tensors (e.g. a rollout slot; either may be None).  Asynchronous."""
         return self._stepper.sample_policy(logits_agent, logits_planner, seed=seed, greedy=greedy, out=out)
 
+    def evaluate_actions(self, logits_agent, logits_planner, actions, masks):
+        """Log-probabilities and entropies of stored actions under the masks they were drawn with, for the update pass:
+        (log_prob_agent, log_prob_planner, entropy_agent, entropy_planner), float32, shaped like the actions (the
+        planner entries are None without planner actions).
+
+        The segments are sample_actions's, and so is the arithmetic: a log-probability is bit for bit what
+        sample_actions returned for the same logits, masks and action.  logits_agent: [*B, A, Na], logits_planner:
+        [*B, Np] (ignored without planner actions), one dtype, float32 or bfloat16; masks = (mask_agent [*B, A, Na],
+        mask_planner [*B, Np]) as the env wrote them (obs_tensors["mask_*"] at sampling time), float32 or bfloat16;
+        actions = (actions_agent [*B, A, n_act], actions_planner [*B, n_act_p]), int32.  *B is any leading shape,
+        e.g. a minibatch of stored rollout steps; every tensor contiguous on the env's device.  Differentiable with
+        respect to both logits tensors: the backward is one device launch that recomputes the softmax.  A segment
+        with nothing open gives 0 and 0 (gradient 0); a NaN or +inf open logit, no finite open logit, or a stored
+        action that is closed gives NaN (see include/aie_b200.h).  Asynchronous; the env's state is not touched."""
+        return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
+
     # ------------------------------------------------------------------ outputs
     @staticmethod
     def _named_fields(flat, layout):

@@ -294,6 +294,14 @@ class CovidBatchedEnv:
         float32: buffers of the env reused by the next call, or the caller's `out` tensors.  Asynchronous."""
         return self._stepper.sample_policy(logits_agent, logits_planner, seed=seed, greedy=greedy, out=out)
 
+    def evaluate_actions(self, logits_agent, logits_planner, actions, masks):
+        """Log-probabilities and entropies of stored actions (the contract of BatchedFoundationEnv.evaluate_actions):
+        logits_agent [*B, 51, 1 + stringency levels], logits_planner [*B, 1 + subsidy levels]; masks = (mask_agent
+        [*B, 1 + levels, 51] as obs["a"]["action_mask"], mask_planner [*B, 1 + subsidy levels]); actions =
+        (actions_agent [*B, 51], actions_planner [*B]), int32.  Returns (log_prob_agent [*B, 51], log_prob_planner
+        [*B], entropy_agent [*B, 51], entropy_planner [*B]), differentiable with respect to both logits tensors."""
+        return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
+
     def _build_views(self):
         b = self._stepper.buf
         S = self.n_agents

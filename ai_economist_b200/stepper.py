@@ -26,6 +26,51 @@ def buf_kind_torch(torch, device, buf):
     return None
 
 
+def is_i32_numpy(buf):
+    return isinstance(buf, np.ndarray) and buf.flags["C_CONTIGUOUS"] and buf.dtype == np.int32
+
+
+def is_i32_torch(torch, device, buf):
+    return isinstance(buf, torch.Tensor) and buf.device == device and buf.is_contiguous() and buf.dtype == torch.int32
+
+
+_EVALUATE_ACTIONS = None
+
+
+def evaluate_actions_function():
+    """The torch.autograd.Function of evaluate_actions (built on first use: torch is imported lazily)."""
+    global _EVALUATE_ACTIONS
+    if _EVALUATE_ACTIONS is not None:
+        return _EVALUATE_ACTIONS
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class EvaluateActions(torch.autograd.Function):
+        """(log_prob_agent, log_prob_planner, entropy_agent, entropy_planner) of stored actions, differentiable with
+        respect to both logits tensors: the backward is one launch of the library's backward kernel on the current
+        stream, which recomputes the softmax from the saved logits and masks."""
+
+        @staticmethod
+        def forward(ctx, stepper, logits_agent, logits_planner, actions_agent, actions_planner, mask_agent, mask_planner):
+            ctx.set_materialize_grads(False)   # an unused output's gradient stays None: a NULL upstream (zero)
+            ctx.stepper = stepper
+            ctx.save_for_backward(logits_agent, logits_planner, actions_agent, actions_planner, mask_agent, mask_planner)
+            return stepper.evaluate_policy(logits_agent, logits_planner, (actions_agent, actions_planner),
+                                           (mask_agent, mask_planner))
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, g_lp_a, g_lp_p, g_h_a, g_h_p):
+            la, lp, aa, ap, ma, mp = ctx.saved_tensors
+            c = lambda g: None if g is None else g.to(torch.float32).contiguous()
+            ga, gp = ctx.stepper.evaluate_policy_backward(la, lp, (aa, ap), (ma, mp), (c(g_lp_a), c(g_lp_p)),
+                                                          (c(g_h_a), c(g_h_p)))
+            return None, ga, gp, None, None, None, None
+
+    _EVALUATE_ACTIONS = EvaluateActions
+    return _EVALUATE_ACTIONS
+
+
 class PolicySampler:
     """sample_policy() of a stepper: a policy's actions drawn on the device from its logits under the env's current
     masks (aie_sample_policy / aie_covid_sample_policy).  The stepper provides _policy_fn (the ABI entry point),
@@ -75,6 +120,115 @@ class PolicySampler:
         p.log_prob_planner = self._ptr(lp_p) if lp_p is not None else None
         self._check(self._policy_fn(self._h, C.byref(p), C.c_uint64(int(seed)), self._stream()))
         return lp_a, lp_p
+
+    # -- evaluation of stored actions (aie_evaluate_policy / aie_covid_evaluate_policy and their backward) -----------
+    def _eval_args(self, logits_agent, logits_planner, actions, masks, grads=()):
+        """Validate the inputs of an evaluation; returns (aie_policy_eval with the inputs set, leading shape, row
+        count, planner?, logits kind, output row shapes).  Raises ValueError before the library is called."""
+        sa, sp, sla, slp = self._policy_shapes()
+        ra, rp, rla = sa[1:], None if sp is None else sp[1:], sla[1:]
+        rlp = None if slp is None else slp[1:]
+        rma, rmp = self._mask_rows()
+        kind = self._buf_kind(logits_agent)
+        shape = tuple(getattr(logits_agent, "shape", ()))
+        if kind is None or len(shape) < len(ra) or shape[len(shape) - len(ra):] != ra:
+            raise ValueError("logits_agent must be a contiguous float32 or bfloat16 [*B, %s] tensor on the env's device"
+                             % ", ".join(map(str, ra)))
+        lead = shape[:len(shape) - len(ra)]
+        tname = "float32" if kind == "f32" else "bfloat16"
+        if not isinstance(actions, (tuple, list)) or len(actions) != 2:
+            raise ValueError("actions must be (actions_agent, actions_planner)")
+        if not isinstance(masks, (tuple, list)) or len(masks) != 2:
+            raise ValueError("masks must be (mask_agent, mask_planner)")
+        mkind = self._buf_kind(masks[0])
+        if mkind is None or tuple(masks[0].shape) != lead + rma:
+            raise ValueError("mask_agent must be a contiguous float32 or bfloat16 %s tensor on the env's device"
+                             % (lead + rma,))
+        if not self._is_i32(actions[0]) or tuple(actions[0].shape) != lead + rla:
+            raise ValueError("actions_agent must be a contiguous int32 %s tensor on the env's device" % (lead + rla,))
+        planner = sp is not None
+        if planner:
+            if logits_planner is None or self._buf_kind(logits_planner) != kind or tuple(logits_planner.shape) != lead + rp:
+                raise ValueError("logits_planner must be a contiguous %s %s tensor on the env's device (the dtype of "
+                                 "logits_agent): this config has planner actions" % (tname, lead + rp))
+            if masks[1] is None or self._buf_kind(masks[1]) != mkind or tuple(masks[1].shape) != lead + rmp:
+                raise ValueError("mask_planner must be a contiguous %s tensor of the dtype of mask_agent on the env's "
+                                 "device" % (lead + rmp,))
+            if not self._is_i32(actions[1]) or tuple(actions[1].shape) != lead + rlp:
+                raise ValueError("actions_planner must be a contiguous int32 %s tensor on the env's device" % (lead + rlp,))
+        for name, (ga, gp) in grads:
+            if ga is not None and (self._buf_kind(ga) != "f32" or tuple(ga.shape) != lead + rla):
+                raise ValueError("%s[0] must be None or a contiguous float32 %s tensor on the env's device" % (name, lead + rla))
+            if planner and gp is not None and (self._buf_kind(gp) != "f32" or tuple(gp.shape) != lead + rlp):
+                raise ValueError("%s[1] must be None or a contiguous float32 %s tensor on the env's device" % (name, lead + rlp))
+        p = _abi.AiePolicyEval()
+        p.logits_agent, p.mask_agent, p.actions_agent = self._ptr(logits_agent), self._ptr(masks[0]), self._ptr(actions[0])
+        if planner:
+            p.logits_planner, p.mask_planner, p.actions_planner = (self._ptr(logits_planner), self._ptr(masks[1]),
+                                                                   self._ptr(actions[1]))
+        p.logits_dtype = _abi.OBS_BF16 if kind == "bf16" else _abi.OBS_F32
+        p.mask_dtype = _abi.OBS_BF16 if mkind == "bf16" else _abi.OBS_F32
+        n = int(np.prod(lead, dtype=np.int64)) if lead else 1
+        return p, lead, n, planner, kind, (ra, rp, rla, rlp)
+
+    def evaluate_policy(self, logits_agent, logits_planner, actions, masks):
+        """Log-probabilities and entropies of stored actions under the masks they were drawn with, per mask segment:
+        (log_prob_agent, log_prob_planner, entropy_agent, entropy_planner), new float32 buffers shaped like the actions
+        (the planner entries are None without planner actions).  Logits: [*B, <the sampler's logits row>], float32 or
+        bfloat16 (raw uint16 bits on numpy backends), both of one dtype; masks = (mask_agent, mask_planner) as the
+        env wrote them ([*B, <mask row>], float32 or bfloat16); actions = (actions_agent, actions_planner), int32
+        [*B, <action row>].  *B is any leading shape (a minibatch of stored steps).  Asynchronous on the stream; no
+        state of the env is read or changed.  Anything else is a ValueError before the library is called."""
+        p, lead, n, planner, _, (_, _, rla, rlp) = self._eval_args(logits_agent, logits_planner, actions, masks)
+        lp_a, h_a = self._eval_out(lead + rla, "f32"), self._eval_out(lead + rla, "f32")
+        lp_p, h_p = (self._eval_out(lead + rlp, "f32"), self._eval_out(lead + rlp, "f32")) if planner else (None, None)
+        p.log_prob_agent, p.entropy_agent = self._ptr(lp_a), self._ptr(h_a)
+        if planner:
+            p.log_prob_planner, p.entropy_planner = self._ptr(lp_p), self._ptr(h_p)
+        self._check(self._eval_fns[0](self._h, C.byref(p), C.c_int64(n), self._stream()))
+        return lp_a, lp_p, h_a, h_p
+
+    def evaluate_policy_backward(self, logits_agent, logits_planner, actions, masks, grad_log_prob=(None, None),
+                                 grad_entropy=(None, None)):
+        """The gradient of sum(g_lp * log_prob + g_H * entropy) with respect to (logits_agent, logits_planner) for
+        the inputs of evaluate_policy; grad_log_prob and grad_entropy = (agent, planner) float32 tensors shaped like
+        the actions, None for zero.  Returns new tensors of the logits' shape and dtype (None for the planner without
+        planner actions).  Asynchronous on the stream."""
+        p, lead, n, planner, kind, (ra, rp, _, _) = self._eval_args(
+            logits_agent, logits_planner, actions, masks, (("grad_log_prob", grad_log_prob), ("grad_entropy", grad_entropy)))
+        ga = self._eval_out(lead + ra, kind)
+        gp = self._eval_out(lead + rp, kind) if planner else None
+        ptr = lambda x: None if x is None else self._ptr(x)
+        p.grad_log_prob_agent, p.grad_entropy_agent, p.grad_logits_agent = ptr(grad_log_prob[0]), ptr(grad_entropy[0]), ptr(ga)
+        if planner:
+            p.grad_log_prob_planner, p.grad_entropy_planner = ptr(grad_log_prob[1]), ptr(grad_entropy[1])
+            p.grad_logits_planner = ptr(gp)
+        self._check(self._eval_fns[1](self._h, C.byref(p), C.c_int64(n), self._stream()))
+        return ga, gp
+
+    def evaluate_actions(self, logits_agent, logits_planner, actions, masks):
+        """evaluate_policy, differentiable with respect to both logits tensors when they are torch tensors (through
+        evaluate_actions_function()); numpy backends call evaluate_policy directly."""
+        if isinstance(logits_agent, np.ndarray):
+            return self.evaluate_policy(logits_agent, logits_planner, actions, masks)
+        planner = self._policy_shapes()[1] is not None
+        if not isinstance(actions, (tuple, list)) or len(actions) != 2:
+            raise ValueError("actions must be (actions_agent, actions_planner)")
+        if not isinstance(masks, (tuple, list)) or len(masks) != 2:
+            raise ValueError("masks must be (mask_agent, mask_planner)")
+        return evaluate_actions_function().apply(self, logits_agent, logits_planner if planner else None, actions[0],
+                                                 actions[1] if planner else None, masks[0], masks[1] if planner else None)
+
+    def _mask_rows(self):
+        """(agent mask row, planner mask row or None): the logits' rows (COVID-19 overrides: its agent mask is transposed)."""
+        sa, sp, _, _ = self._policy_shapes()
+        return sa[1:], None if sp is None else sp[1:]
+
+    def _eval_out(self, shape, kind):
+        return np.empty(shape, {"f32": np.float32, "bf16": np.uint16}[kind])
+
+    def _is_i32(self, buf):
+        return is_i32_numpy(buf)
 
     def _buf_kind(self, buf):
         return buf_kind_numpy(buf)
@@ -342,6 +496,10 @@ class BatchStepper(PolicySampler):
     def _policy_fn(self):
         return self.lib.aie_sample_policy
 
+    @property
+    def _eval_fns(self):
+        return self.lib.aie_evaluate_policy, self.lib.aie_evaluate_policy_backward
+
     def _policy_shapes(self):
         d, E, A = self.dims, self.n_envs, self.spec["n_agents"]
         has_p = d.n_act_planner > 0
@@ -477,6 +635,12 @@ class CudaStepper(BatchStepper):
         t = self.torch
         return (isinstance(buf, t.Tensor) and buf.dtype == like.dtype and buf.shape == like.shape and buf.is_contiguous()
                 and buf.device == self.device)
+
+    def _is_i32(self, buf):
+        return is_i32_torch(self.torch, self.device, buf)
+
+    def _eval_out(self, shape, kind):
+        return self._empty(shape, kind)
 
     def _buf_kind(self, buf):
         return buf_kind_torch(self.torch, self.device, buf)

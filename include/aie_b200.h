@@ -422,6 +422,49 @@ typedef struct aie_policy_logits {
  * and state is loaded. */
 int aie_sample_policy(aie_env *env, const aie_policy_logits *p, uint64_t seed, void *stream);
 
+/* Stored actions of a policy and the masks they were drawn under, for the update pass: N rows, each laid out like one
+ * env's logits, masks and actions (a PPO minibatch of rollout steps, any N).  DEVICE pointers; "planner" entries are
+ * NULL / ignored when the config has no planner actions. */
+typedef struct aie_policy_eval {
+    const void *logits_agent;             /* [N, A, Na] (the layout of aie_policy_logits::agent); COVID-19 [N, S, 1 + levels] */
+    const void *logits_planner;           /* [N, Np]; COVID-19 [N, 1 + subsidy levels] */
+    const void *mask_agent;               /* [N, A, Na] as the env wrote mask_agent; COVID-19 [N, 1 + levels, S] */
+    const void *mask_planner;             /* [N, Np]; COVID-19 [N, 1 + subsidy levels] */
+    const int32_t *actions_agent;         /* [N, A, n_act_a]; COVID-19 [N, S] */
+    const int32_t *actions_planner;       /* [N, n_act_p]; COVID-19 [N] */
+    int32_t logits_dtype;                 /* AIE_OBS_F32 | AIE_OBS_BF16: both logits tensors and both gradients */
+    int32_t mask_dtype;                   /* AIE_OBS_F32 | AIE_OBS_BF16: both masks */
+    float *log_prob_agent, *log_prob_planner;    /* forward outputs, shaped like the actions */
+    float *entropy_agent, *entropy_planner;      /* forward outputs, shaped like the actions */
+    const float *grad_log_prob_agent, *grad_log_prob_planner;   /* backward: upstream gradients, NULL = zero */
+    const float *grad_entropy_agent, *grad_entropy_planner;     /* backward: upstream gradients, NULL = zero */
+    void *grad_logits_agent, *grad_logits_planner;              /* backward outputs: the logits' layout and dtype */
+} aie_policy_eval;
+
+/* ABI 5.  Log-probabilities and entropies of stored actions: per row and mask segment (the sampler's segments: a
+ * single-action agent's whole row, each multi-action subspace with its own NO-OP, each planner bracket or the
+ * single-action planner's one index), with m = the largest open logit, w_j = exp((double)l_j - m) for open j,
+ * Z = sum w_j (accumulated in aie_sample_policy's order), p_j = w_j / Z, a = the stored action, in float64 and rounded once:
+ *   log_prob = (float)(((double)l_a - m) - log(Z))   - bit for bit what aie_sample_policy returned for the same logits,
+ *                                                      masks and action on the same backend;
+ *   entropy  = (float)(log(Z) - sum_j p_j ((double)l_j - m)).
+ * A segment with no open entry: 0 and 0.  An open logit that is NaN or +inf, or no finite open logit: NaN and NaN.
+ * An action that is closed or outside [0, n): log_prob NaN, the entropy as usual.
+ * One launch, asynchronous on `stream`; N = 0 is a no-op.  It reads no env record and needs no bound buffers or loaded
+ * state (only the config), and moves no counter of the env.  AIE_EINVAL for a NULL p, a negative N, an unknown
+ * logits_dtype or mask_dtype, and (N > 0) a NULL required pointer (the logits, masks, actions and outputs of the agents,
+ * and of the planner when the config has planner actions) or a pointer not aligned to its element size. */
+int aie_evaluate_policy(aie_env *env, const aie_policy_eval *p, int64_t n_rows, void *stream);
+/* ABI 5.  The gradient of sum(g_lp * log_prob + g_H * entropy) with respect to the logits (the backward of
+ * aie_evaluate_policy; m and Z recomputed from the logits), into grad_logits_*, every entry written: for open j
+ *   g_lp ([j = a] - p_j) - g_H p_j (((double)l_j - m - log(Z)) + H)   (H the float64 entropy; an open entry with
+ *                                                                     p_j = 0 has no g_H term),
+ * 0 for closed entries.  A segment with no open entry: 0.  An open logit that is NaN or +inf, no finite open logit, or
+ * a stored action that is closed or outside [0, n): NaN at the open entries, 0 at the closed ones.  bfloat16 gradients
+ * are the round-to-nearest-even of the float64 value.  The outputs of aie_evaluate_policy are neither read nor needed
+ * (log_prob_* / entropy_* may be NULL); grad_logits_* are required instead.  Errors as aie_evaluate_policy. */
+int aie_evaluate_policy_backward(aie_env *env, const aie_policy_eval *p, int64_t n_rows, void *stream);
+
 /* End-to-end variant with HOST buffers: copies the actions host->device, steps, copies every non-NULL
  * output device->host, and synchronises the stream.  Buffers should be pinned for full PCIe rate. */
 int aie_step_host(aie_env *env, const int32_t *actions_agent_host, const int32_t *actions_planner_host,
@@ -559,6 +602,12 @@ int aie_covid_sample_random_actions(aie_covid_env *env, uint64_t seed, void *str
  * with s = host_mix64(seed) ^ host_mix64(n), n counting this env's aie_covid_sample_policy calls; state a draws with
  * k + 0x100 * a, the planner with k ^ 0xabcdef.  AIE_EINVAL also when 1 + subsidy levels > 160. */
 int aie_covid_sample_policy(aie_covid_env *env, const aie_policy_logits *p, uint64_t seed, void *stream);
+/* Log-probabilities, entropies and their gradient for stored actions (the contract of aie_evaluate_policy /
+ * aie_evaluate_policy_backward): agent logits [N, S, 1 + levels] read against masks [N, 1 + levels, S], planner logits
+ * and masks [N, 1 + subsidy levels] (required), actions [N, S] and [N]; outputs shaped like the actions.
+ * AIE_EINVAL also when 1 + subsidy levels > 160. */
+int aie_covid_evaluate_policy(aie_covid_env *env, const aie_policy_eval *p, int64_t n_rows, void *stream);
+int aie_covid_evaluate_policy_backward(aie_covid_env *env, const aie_policy_eval *p, int64_t n_rows, void *stream);
 int64_t aie_covid_launch_count(const aie_covid_env *env);
 
 const char *aie_last_error(void);
