@@ -8,6 +8,7 @@ ABI_VERSION = 5
 MAX_COMPONENTS, MAX_BRACKETS, MAX_RATES = 8, 16, 64
 AIE_OK = 0
 OBS_F32, OBS_BF16 = 0, 1   # aie_config.obs_dtype
+REWARD_F32, REWARD_F64 = 0, 1   # aie_advantage_args.rewards_*_dtype
 
 COMPONENT_KIND = {"Build": 0, "ContinuousDoubleAuction": 1, "Gather": 2, "PeriodicBracketTax": 3,
                   "WealthRedistribution": 4, "SimpleLabor": 5}
@@ -135,6 +136,15 @@ class AiePolicyEval(C.Structure):
                                              "grad_entropy_planner", "grad_logits_agent", "grad_logits_planner"]])
 
 
+class AieAdvantageArgs(C.Structure):
+    _fields_ = ([("rewards_agent", C.c_void_p), ("rewards_planner", C.c_void_p), ("rewards_agent_dtype", C.c_int32),
+                 ("rewards_planner_dtype", C.c_int32)]
+                + [(n, C.c_void_p) for n in ["values_agent", "values_planner", "dones", "last_values_agent",
+                                             "last_values_planner", "final_values_agent", "final_values_planner"]]
+                + [(n, C.c_double) for n in ["gamma_agent", "gamma_planner", "lambda_agent", "lambda_planner"]]
+                + [(n, C.c_void_p) for n in ["adv_agent", "adv_planner", "ret_agent", "ret_planner"]])
+
+
 class AieCovidConfig(C.Structure):
     _fields_ = ([(n, C.c_int32) for n in [
         "abi_version", "n_states", "episode_length", "num_stringency_levels", "action_cooldown_period",
@@ -204,6 +214,9 @@ def load_library(path=None):
                "aie_covid_evaluate_policy_backward"]:
         getattr(L, fn).argtypes = [P, C.POINTER(AiePolicyEval), C.c_int64, P]
         getattr(L, fn).restype = C.c_int
+    for fn in ["aie_compute_advantages", "aie_covid_compute_advantages"]:
+        getattr(L, fn).argtypes = [P, C.POINTER(AieAdvantageArgs), C.c_int32, P]
+        getattr(L, fn).restype = C.c_int
     L.aie_step_host.argtypes = [P, P, P, C.POINTER(AieHostOut), P]
     L.aie_step_host_compact.argtypes = [P, P, P, C.POINTER(AieHostOut), C.c_int32, P]
     L.aie_step_host_compact.restype = C.c_int
@@ -242,11 +255,11 @@ def load_library(path=None):
 
 EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field", "aie_get_flat_layout", "aie_bind_buffers",
                     "aie_load_state", "aie_reset_envs", "aie_step", "aie_step_dynamics", "aie_observe", "aie_observe_final", "aie_sample_random_actions",
-                    "aie_set_fused_policy", "aie_sample_policy", "aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
+                    "aie_set_fused_policy", "aie_sample_policy", "aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_compute_advantages", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
                     "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
                     "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
-                    "aie_covid_evaluate_policy_backward", "aie_covid_launch_count"]
+                    "aie_covid_evaluate_policy_backward", "aie_covid_compute_advantages", "aie_covid_launch_count"]
 
 
 def obs_dtype_name(obs_dtype):

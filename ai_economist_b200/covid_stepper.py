@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from .stepper import PolicySampler, buf_kind_torch, is_i32_torch
+from .stepper import PolicySampler, buf_kind_torch, float_kind_torch, is_i32_torch
 
 F32, I32 = np.float32, np.int32
 
@@ -145,6 +145,10 @@ class CovidStepperBase(PolicySampler):
     def _eval_fns(self):
         return self.lib.aie_covid_evaluate_policy, self.lib.aie_covid_evaluate_policy_backward
 
+    @property
+    def _adv_fn(self):
+        return self.lib.aie_covid_compute_advantages
+
     def _mask_rows(self):   # evaluate_policy: the agent mask is [*B, 1 + levels, S], transposed against the logits
         S, L = self.p["n_states"], self.p["num_stringency_levels"]
         return (1 + L, S), (1 + self.p["num_subsidy_levels"],)
@@ -192,6 +196,9 @@ class CudaCovidStepper(CovidStepperBase):
 
     def _is_i32(self, buf):
         return is_i32_torch(self.torch, self.device, buf)
+
+    def _float_kind(self, buf):
+        return float_kind_torch(self.torch, self.device, buf)
 
     def _eval_out(self, shape, kind):
         t = self.torch

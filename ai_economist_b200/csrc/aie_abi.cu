@@ -22,6 +22,8 @@
 //                          (aie_evaluate_policy_backward); instantiated for float32 / bfloat16 masks and logits.
 //   aie_covid_evaluate_policy_kernel, aie_covid_evaluate_policy_backward_kernel  one warp per (row, state | planner):
 //                          the same for the COVID-19 scenario.
+//   aie_compute_advantages_kernel  one thread per column of a stored rollout (agent and planner columns, group-uniform
+//                          CTAs): advantages and value targets (aie_compute_advantages, aie_covid_compute_advantages).
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
 // aie_config::obs_dtype == AIE_OBS_BF16); the launchers pick one from the config, with the same launch shape.
 #include <cuda_runtime.h>
@@ -110,6 +112,7 @@ int covid_launch_policy(aie_covid_env *, const PolicyBufs &p, int lt_bf16, uint6
 int launch_policy_eval(aie_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows, void *stream);
 int covid_launch_policy_eval(aie_covid_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows,
                              void *stream);
+int launch_advantages(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, void *stream);
 }  // namespace be
 }  // namespace aie
 
@@ -1095,6 +1098,38 @@ int covid_launch_step(aie_covid_env *env, void *stream) {
     aie_covid_step_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     AIE_CUDA(cudaGetLastError(), "aie_covid_step_kernel launch");
     env->launches++;
+    return AIE_OK;
+}
+}  // namespace be
+}  // namespace aie
+
+// ---------------------------------------------------------------------------------------------------------
+namespace aie {
+// Advantages of a stored rollout (aie_compute_advantages): one thread per column, the agents' columns in the first
+// cta_a CTAs and the planner's after them, so each warp reads one group's rows coalesced along the column at every t.
+template <typename RA, typename RP>
+__global__ void __launch_bounds__(256) aie_compute_advantages_kernel(const __grid_constant__ AdvantageBufs b, long long E,
+                                                                     int T, unsigned cta_a) {
+    if (blockIdx.x < cta_a) {
+        const long long col = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+        if (col < b.n[0]) gae_column<RA>(b, 0, E, col, T);
+    } else {
+        const long long col = (long long)(blockIdx.x - cta_a) * blockDim.x + threadIdx.x;
+        if (col < b.n[1]) gae_column<RP>(b, 1, E, col, T);
+    }
+}
+namespace be {
+int launch_advantages(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, void *stream) {
+    const long long cta_a = (b.n[0] + 255) / 256, cta_p = (b.n[1] + 255) / 256;
+    if (cta_a + cta_p > 0x7fffffffLL) return fail(AIE_EINVAL, "aie_compute_advantages: too many columns for one launch");
+    const unsigned grid = (unsigned)(cta_a + cta_p), ca = (unsigned)cta_a;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (ra64) {
+        if (rp64) aie_compute_advantages_kernel<double, double><<<grid, 256, 0, st>>>(b, E, T, ca);
+        else aie_compute_advantages_kernel<double, float><<<grid, 256, 0, st>>>(b, E, T, ca);
+    } else if (rp64) aie_compute_advantages_kernel<float, double><<<grid, 256, 0, st>>>(b, E, T, ca);
+    else aie_compute_advantages_kernel<float, float><<<grid, 256, 0, st>>>(b, E, T, ca);
+    AIE_CUDA(cudaGetLastError(), "aie_compute_advantages_kernel launch");
     return AIE_OK;
 }
 }  // namespace be

@@ -2007,4 +2007,89 @@ AIE_DEV void policy_eval_row(const DevCfg &c, const PolicyEvalBufs &p, long long
     for (int v = 0; v < units; v++) policy_eval_unit<BWD, MT, LT>(c, p, r, v, lane);
 }
 
+// Where aie_compute_advantages reads and writes: group g = 0 the agents' columns ([T][E * A]), g = 1 the planner's ([T][E]).
+struct AdvantageBufs {
+    const void *r[2];                 // rewards, float or double (the kernel's template arguments)
+    const float *v[2], *lv[2], *fv[2];   // values [T][n], last values [n], final values [T][n] or null
+    const int32_t *done;              // [T][E]
+    float *adv[2], *ret[2];           // [T][n]
+    double gamma[2], gl[2];           // gl = gamma * lambda
+    long long n[2];                   // columns: E * A, E (0: no planner group)
+    int per_env[2];                   // columns per env: A, 1
+};
+// Timesteps per chunk of a column's loads: the loads of the next chunk are issued before the current one is computed,
+// and they do not depend on the carry, so a column keeps 2 * AIE_GAE_K timesteps of loads in flight.
+#ifndef AIE_GAE_K
+#define AIE_GAE_K 8
+#endif
+#if AIE_ON_DEVICE
+#define AIE_GAE_UNROLL AIE_UNROLL(AIE_GAE_K)
+#else
+#define AIE_GAE_UNROLL
+#endif
+// The dones of the chunk ending at row hi - 1 (rows hi - AIE_GAE_K .. hi - 1 read backwards; rows < 0 are 0).
+AIE_DEV void gae_load_done(int32_t *d, const int32_t *done, long long E, long long e, int hi) {
+    AIE_GAE_UNROLL
+    for (int k = 0; k < AIE_GAE_K; k++) {
+        const int t = hi - 1 - k;
+        d[k] = t >= 0 ? done[(long long)t * E + e] : 0;
+    }
+}
+// Rewards, values and (where the done holds) final values of the same chunk.
+template <typename RT>
+AIE_DEV void gae_load_vals(RT *r, float *v, float *f, const int32_t *d, const RT *R, const float *V, const float *F,
+                           long long n, long long col, int hi) {
+    AIE_GAE_UNROLL
+    for (int k = 0; k < AIE_GAE_K; k++) {
+        const int t = hi - 1 - k;
+        const long long i = (long long)t * n + col;
+        r[k] = t >= 0 ? R[i] : (RT)0;
+        v[k] = t >= 0 ? V[i] : 0.f;
+        f[k] = (t >= 0 && F && d[k]) ? F[i] : 0.f;
+    }
+}
+// One column of group g over T steps (the recursion of aie_compute_advantages, include/aie_b200.h).  The carry is
+// only A and the value of the next row; the dones run one chunk ahead of the other loads so that the final values of
+// a chunk can be fetched as soon as its rewards and values are.
+template <typename RT>
+AIE_DEV void gae_column(const AdvantageBufs &b, int g, long long E, long long col, int T) {
+    constexpr int K = AIE_GAE_K;
+    const long long n = b.n[g], e = col / b.per_env[g];
+    const RT *R = (const RT *)b.r[g];
+    const float *V = b.v[g], *F = b.fv[g];
+    const double gamma = b.gamma[g], gl = b.gl[g];
+    int32_t dn[K], dnn[K];
+    RT rn[K];
+    float vn[K], fn[K];
+    gae_load_done(dn, b.done, E, e, T);
+    gae_load_vals<RT>(rn, vn, fn, dn, R, V, F, n, col, T);
+    gae_load_done(dnn, b.done, E, e, T - K);
+    float vnext = b.lv[g][col];
+    double a = 0.0;
+    for (int hi = T; hi > 0; hi -= K) {
+        int32_t d[K];
+        RT r[K];
+        float v[K], f[K];
+        AIE_GAE_UNROLL
+        for (int k = 0; k < K; k++) { d[k] = dn[k]; r[k] = rn[k]; v[k] = vn[k]; f[k] = fn[k]; dn[k] = dnn[k]; }
+        if (hi - K > 0) {
+            gae_load_vals<RT>(rn, vn, fn, dn, R, V, F, n, col, hi - K);
+            gae_load_done(dnn, b.done, E, e, hi - 2 * K);
+        }
+        AIE_GAE_UNROLL
+        for (int k = 0; k < K; k++) {
+            const int t = hi - 1 - k;
+            if (t < 0) break;
+            const bool dk = d[k] != 0;
+            const double nv = dk ? (double)f[k] : (double)vnext;
+            const double delta = ((double)r[k] + gamma * nv) - (double)v[k];
+            a = (dk || t == T - 1) ? delta : delta + gl * a;
+            const long long i = (long long)t * n + col;
+            b.adv[g][i] = (float)a;
+            b.ret[g][i] = (float)(a + (double)v[k]);
+            vnext = v[k];
+        }
+    }
+}
+
 }  // namespace aie

@@ -593,6 +593,23 @@ class BatchedFoundationEnv:
         action that is closed gives NaN (see include/aie_b200.h).  Asynchronous; the env's state is not touched."""
         return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
 
+    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0):
+        """Advantages and value targets of a stored rollout of T steps (generalised advantage estimation), bootstrapped
+        at episode ends: (adv_agent [T, E, A], adv_planner [T, E], ret_agent, ret_planner), float32, one device launch.
+
+        rewards = (agent [T, E, A], planner [T, E]) as the env wrote them after each step (rew["a"] / rew["p"] with
+        collated data), float32 or float64; values = (agent, planner), float32, the value of the observation each
+        step's action was taken from; dones = int32 [T, E], done["__all__"] after each step; last_values = (agent
+        [E, A], planner [E]), float32, the value of the observation after the last step.  Every episode here ends on its
+        time limit, and the auto-reset hands back the next episode's observation at the step that ends one, so the
+        target of a done step should bootstrap from the value of that step's env.final_obs: pass those values as
+        final_values = (agent, planner) shaped like values (rows where dones is 0 are never read, so the value net's
+        output over the whole final_obs tensor will do).  final_values=None treats an episode end as terminal.  gamma,
+        lam: floats in [0, 1] or (agents, planner) pairs.  The planner entries may be None together (a trainer without
+        a planner policy; its outputs are then None).  Computed in float64 exactly as include/aie_b200.h spells out.
+        Every tensor contiguous on the env's device; asynchronous on the current stream; the env's state is not touched."""
+        return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam)
+
     # ------------------------------------------------------------------ outputs
     @staticmethod
     def _named_fields(flat, layout):

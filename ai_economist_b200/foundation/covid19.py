@@ -302,6 +302,13 @@ class CovidBatchedEnv:
         [*B], entropy_agent [*B, 51], entropy_planner [*B]), differentiable with respect to both logits tensors."""
         return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
 
+    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0):
+        """Advantages and value targets of a stored rollout (the contract of BatchedFoundationEnv.compute_advantages),
+        A = 51 states: rewards = (rew["a"] [T, E, 51] float32, rew["p"] [T, E] float64) stacked over the steps, values
+        = (agent, planner) float32 of the same shapes, dones int32 [T, E], last_values = ([E, 51], [E]).  This env has
+        no final observations yet, so final_values is normally None: an episode end is then treated as terminal."""
+        return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam)
+
     def _build_views(self):
         b = self._stepper.buf
         S = self.n_agents

@@ -1,6 +1,7 @@
 """Thin Python driver over the C-ABI: allocates the device buffers (PyTorch-owned), binds them, uploads host
 reset snapshots and launches steps.  Plumbing only — all compute is in the CUDA library."""
 import ctypes as C
+import numbers
 
 import numpy as np
 
@@ -23,6 +24,20 @@ def buf_kind_torch(torch, device, buf):
     """"f32" / "bf16" for a contiguous float32 / bfloat16 tensor on `device`, else None."""
     if isinstance(buf, torch.Tensor) and buf.device == device and buf.is_contiguous():
         return {torch.float32: "f32", torch.bfloat16: "bf16"}.get(buf.dtype)
+    return None
+
+
+def float_kind_numpy(buf):
+    """"f32" / "f64" for a C-contiguous float32 / float64 numpy array, else None."""
+    if isinstance(buf, np.ndarray) and buf.flags["C_CONTIGUOUS"]:
+        return {np.dtype(np.float32): "f32", np.dtype(np.float64): "f64"}.get(buf.dtype)
+    return None
+
+
+def float_kind_torch(torch, device, buf):
+    """"f32" / "f64" for a contiguous float32 / float64 tensor on `device`, else None."""
+    if isinstance(buf, torch.Tensor) and buf.device == device and buf.is_contiguous():
+        return {torch.float32: "f32", torch.float64: "f64"}.get(buf.dtype)
     return None
 
 
@@ -219,6 +234,88 @@ class PolicySampler:
         return evaluate_actions_function().apply(self, logits_agent, logits_planner if planner else None, actions[0],
                                                  actions[1] if planner else None, masks[0], masks[1] if planner else None)
 
+    # -- advantages of a stored rollout (aie_compute_advantages / aie_covid_compute_advantages) -----------------------
+    @staticmethod
+    def _discount_pair(x, name, planner):
+        """(agent, planner) of a gamma or lambda given as a float or a pair; each a float in [0, 1]."""
+        pair = tuple(x) if isinstance(x, (tuple, list)) else (x, x)
+        if len(pair) != 2:
+            raise ValueError("%s must be a float or an (agents, planner) pair" % name)
+        out = []
+        for k, v in enumerate(pair):
+            if k == 1 and not planner:
+                out.append(0.0)
+                continue
+            if isinstance(v, bool) or not isinstance(v, numbers.Real):
+                raise ValueError("%s must be a float or an (agents, planner) pair of floats" % name)
+            if not 0.0 <= float(v) <= 1.0:   # NaN fails both comparisons
+                raise ValueError("%s must lie in [0, 1], got %r" % (name, v))
+            out.append(float(v))
+        return out
+
+    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0):
+        """Generalised advantage estimates and value targets of a stored rollout of T steps, bootstrapped at episode
+        ends: (adv_agent, adv_planner, ret_agent, ret_planner), new float32 buffers shaped like the rewards.  rewards =
+        (agent [T, E, A], planner [T, E]), float32 or float64 each; values = (agent, planner), float32 like the
+        rewards; dones int32 [T, E]; last_values = (agent [E, A], planner [E]), float32; final_values None (an episode
+        end is terminal) or (agent, planner) like values, read only where dones is set.  gamma, lam: floats in
+        [0, 1], or (agents, planner) pairs.  Every planner entry may be None together (no planner outputs).  The
+        recursion and its float64 rounding are spelled out in include/aie_b200.h.  Asynchronous on the stream; no
+        state of the env is read or changed.  Anything else is a ValueError before the library is called."""
+        sa = self._policy_shapes()[0]
+        E, A = sa[0], sa[1]
+        pairs = dict(rewards=rewards, values=values, last_values=last_values)
+        if final_values is not None:
+            pairs["final_values"] = final_values
+        for name, x in pairs.items():
+            if not isinstance(x, (tuple, list)) or len(x) != 2:
+                raise ValueError("%s must be an (agent, planner) pair" % name)
+        planner = rewards[1] is not None
+        if any((x[1] is not None) != planner for x in pairs.values()):
+            raise ValueError("the planner entries of rewards, values, last_values and final_values must be all given "
+                             "or all None")
+        shape_a = tuple(getattr(rewards[0], "shape", ()))
+        if len(shape_a) != 3 or shape_a[1:] != (E, A):
+            raise ValueError("rewards[0] must be a [T, %d, %d] tensor" % (E, A))
+        T = shape_a[0]
+        if T > 0x7FFFFFFF:
+            raise ValueError("T must fit in int32")
+        rows = ((T, E, A), (T, E))
+        rk = []
+        for k, who in enumerate(("agent", "planner")[:2 if planner else 1]):
+            kind = self._float_kind(rewards[k])
+            if kind is None or tuple(rewards[k].shape) != rows[k]:
+                raise ValueError("rewards[%d] (%s) must be a contiguous float32 or float64 %s tensor on the env's device"
+                                 % (k, who, rows[k]))
+            rk.append(kind)
+            for name, want in (("values", rows[k]), ("last_values", rows[k][1:]), ("final_values", rows[k])):
+                if name in pairs and (self._float_kind(pairs[name][k]) != "f32" or tuple(pairs[name][k].shape) != want):
+                    raise ValueError("%s[%d] (%s) must be a contiguous float32 %s tensor on the env's device"
+                                     % (name, k, who, want))
+        if not self._is_i32(dones) or tuple(dones.shape) != (T, E):
+            raise ValueError("dones must be a contiguous int32 %s tensor on the env's device" % ((T, E),))
+        g, l = self._discount_pair(gamma, "gamma", planner), self._discount_pair(lam, "lam", planner)
+        q = _abi.AieAdvantageArgs()
+        q.rewards_agent, q.values_agent, q.last_values_agent = self._ptr(rewards[0]), self._ptr(values[0]), self._ptr(last_values[0])
+        q.rewards_agent_dtype = _abi.REWARD_F64 if rk[0] == "f64" else _abi.REWARD_F32
+        q.dones = self._ptr(dones)
+        q.gamma_agent, q.gamma_planner, q.lambda_agent, q.lambda_planner = g[0], g[1], l[0], l[1]
+        adv_a, ret_a = self._eval_out(rows[0], "f32"), self._eval_out(rows[0], "f32")
+        q.adv_agent, q.ret_agent = self._ptr(adv_a), self._ptr(ret_a)
+        adv_p = ret_p = None
+        if planner:
+            q.rewards_planner, q.values_planner = self._ptr(rewards[1]), self._ptr(values[1])
+            q.last_values_planner = self._ptr(last_values[1])
+            q.rewards_planner_dtype = _abi.REWARD_F64 if rk[1] == "f64" else _abi.REWARD_F32
+            adv_p, ret_p = self._eval_out(rows[1], "f32"), self._eval_out(rows[1], "f32")
+            q.adv_planner, q.ret_planner = self._ptr(adv_p), self._ptr(ret_p)
+        if final_values is not None:
+            q.final_values_agent = self._ptr(final_values[0])
+            if planner:
+                q.final_values_planner = self._ptr(final_values[1])
+        self._check(self._adv_fn(self._h, C.byref(q), C.c_int32(T), self._stream()))
+        return adv_a, adv_p, ret_a, ret_p
+
     def _mask_rows(self):
         """(agent mask row, planner mask row or None): the logits' rows (COVID-19 overrides: its agent mask is transposed)."""
         sa, sp, _, _ = self._policy_shapes()
@@ -229,6 +326,9 @@ class PolicySampler:
 
     def _is_i32(self, buf):
         return is_i32_numpy(buf)
+
+    def _float_kind(self, buf):
+        return float_kind_numpy(buf)
 
     def _buf_kind(self, buf):
         return buf_kind_numpy(buf)
@@ -500,6 +600,10 @@ class BatchStepper(PolicySampler):
     def _eval_fns(self):
         return self.lib.aie_evaluate_policy, self.lib.aie_evaluate_policy_backward
 
+    @property
+    def _adv_fn(self):
+        return self.lib.aie_compute_advantages
+
     def _policy_shapes(self):
         d, E, A = self.dims, self.n_envs, self.spec["n_agents"]
         has_p = d.n_act_planner > 0
@@ -638,6 +742,9 @@ class CudaStepper(BatchStepper):
 
     def _is_i32(self, buf):
         return is_i32_torch(self.torch, self.device, buf)
+
+    def _float_kind(self, buf):
+        return float_kind_torch(self.torch, self.device, buf)
 
     def _eval_out(self, shape, kind):
         return self._empty(shape, kind)

@@ -465,6 +465,47 @@ int aie_evaluate_policy(aie_env *env, const aie_policy_eval *p, int64_t n_rows, 
  * (log_prob_* / entropy_* may be NULL); grad_logits_* are required instead.  Errors as aie_evaluate_policy. */
 int aie_evaluate_policy_backward(aie_env *env, const aie_policy_eval *p, int64_t n_rows, void *stream);
 
+/* A stored rollout of T steps of the E replicas, for advantages and value targets: two groups of columns, the agents'
+ * ([T, E, A]: COVID-19 A = S states) and the planner's ([T, E]).  DEVICE pointers, contiguous. */
+enum { AIE_REWARD_F32 = 0, AIE_REWARD_F64 = 1 };
+typedef struct aie_advantage_args {
+    const void *rewards_agent;                /* [T, E, A], as the env wrote its rewards after each step */
+    const void *rewards_planner;              /* [T, E], or NULL: no planner group (its other entries are then ignored) */
+    int32_t rewards_agent_dtype;              /* AIE_REWARD_F32 | AIE_REWARD_F64 */
+    int32_t rewards_planner_dtype;
+    const float *values_agent, *values_planner;             /* [T, E, A], [T, E]: the value of the observation each
+                                                               step's action was taken from */
+    const int32_t *dones;                                    /* [T, E]: done["__all__"] after each step */
+    const float *last_values_agent, *last_values_planner;   /* [E, A], [E]: the value of the observation after step T-1 */
+    const float *final_values_agent, *final_values_planner; /* like values (the value of final_obs after each step), or
+                                                               NULL: an episode end is terminal */
+    double gamma_agent, gamma_planner;        /* each in [0, 1] */
+    double lambda_agent, lambda_planner;      /* each in [0, 1] */
+    float *adv_agent, *adv_planner;           /* outputs, like the rewards */
+    float *ret_agent, *ret_planner;           /* outputs, like the rewards */
+} aie_advantage_args;
+
+/* ABI 5.  Generalised advantage estimation over a stored rollout, bootstrapped at episode ends.  For every column (agent
+ * (e, a) or planner e) of a group with discount gamma and lambda lam, in float64 with every operation rounded (no fused
+ * multiply-add), gl = gamma * lam computed once, R the rewards, V the values, F the final values, LV the last values:
+ *   for t = T-1 .. 0:
+ *       d     = dones[t, e] != 0
+ *       nv    = d ? (F given ? F[t] : 0) : (t == T-1 ? LV : V[t+1])
+ *       delta = (R[t] + gamma * nv) - V[t]
+ *       A     = (d || t == T-1) ? delta : delta + gl * A_next        (the chain is cut, not multiplied by 0)
+ *       adv[t] = (float)A;  ret[t] = (float)(A + V[t])
+ * Under the auto-reset the step that ends an episode returns that episode's reward and done but the next episode's
+ * observation, and every episode ends on its time limit (truncated, not terminal): the target at a done step bootstraps
+ * from the value of that step's final observation (env.final_obs), which F supplies.  F is read only where d holds, so it
+ * may be the value net's output over the whole final-observation tensor, unspecified rows included; without F an episode
+ * end is treated as terminal.  A NaN propagates backwards through its chain up to the previous cut.  The CUDA kernel
+ * and a host build of the same source give the same bits.  One launch, asynchronous on `stream`; T = 0 is a no-op.  It
+ * reads no env record, needs no bound buffers or loaded state (only E and A), and moves no counter of the env.
+ * AIE_EINVAL for a NULL args, a negative T, an unknown reward dtype, a gamma or lambda that is NaN or outside [0, 1],
+ * and (T > 0) a NULL required pointer (every pointer of a group but its final values) or a pointer not aligned to its
+ * element size. */
+int aie_compute_advantages(aie_env *env, const aie_advantage_args *args, int32_t T, void *stream);
+
 /* End-to-end variant with HOST buffers: copies the actions host->device, steps, copies every non-NULL
  * output device->host, and synchronises the stream.  Buffers should be pinned for full PCIe rate. */
 int aie_step_host(aie_env *env, const int32_t *actions_agent_host, const int32_t *actions_planner_host,
@@ -608,6 +649,8 @@ int aie_covid_sample_policy(aie_covid_env *env, const aie_policy_logits *p, uint
  * AIE_EINVAL also when 1 + subsidy levels > 160. */
 int aie_covid_evaluate_policy(aie_covid_env *env, const aie_policy_eval *p, int64_t n_rows, void *stream);
 int aie_covid_evaluate_policy_backward(aie_covid_env *env, const aie_policy_eval *p, int64_t n_rows, void *stream);
+/* Advantages and value targets of a stored rollout (the contract of aie_compute_advantages), A = S states. */
+int aie_covid_compute_advantages(aie_covid_env *env, const aie_advantage_args *args, int32_t T, void *stream);
 int64_t aie_covid_launch_count(const aie_covid_env *env);
 
 const char *aie_last_error(void);
