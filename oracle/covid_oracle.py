@@ -25,8 +25,12 @@ def _softplus(x, beta=1, threshold=20):
 
 
 class CovidOracleEnv:
-    def __init__(self, params):
+    def __init__(self, params, auto_reset=False):
+        # auto_reset: a step that ends the episode resets the env, as the product's auto-reset does: the observations are
+        # the fresh episode's, the rewards and `done` those of the step that ended the finished one
         self.p = params
+        self.auto_reset = auto_reset
+        self.episodes = 0
         self.reset()
 
     def reset(self):
@@ -47,6 +51,7 @@ class CovidOracleEnv:
         self.vaccines_available = np.zeros(S, dtype=np.int64)
         self.rew_a = np.zeros(S, dtype=F32)
         self.rew_p = 0.0
+        self.done = 0
 
     # ------------------------------------------------------------------ step
     def step(self, act_a, act_p):
@@ -95,6 +100,12 @@ class CovidOracleEnv:
         productivity = self._economy(I_t, D_t, unemployed)
         gs["Postsubsidy Productivity"][t] = productivity + gs["Subsidy"][t]
         self._reward()
+        self.done = int(t >= p["episode_length"])
+        if self.auto_reset and self.done:
+            rew_a, rew_p = self.rew_a, self.rew_p
+            self.reset()
+            self.rew_a, self.rew_p, self.done = rew_a, rew_p, 1
+            self.episodes += 1
         return self.obs()
 
     def _sir(self, S_tm1, I_tm1, tmk, vacc_avail):
@@ -188,7 +199,7 @@ class CovidOracleEnv:
             policy_ind=np.asarray(policy_ind, F32),
             scalars=np.array([t / p["time_scale"], t_until_sub, sub_level, t_vac], F32),
             mask_a=mask_a, mask_p=mask_p, rew_a=np.asarray(self.rew_a, F32), rew_p=np.float64(self.rew_p),
-            done=np.int32(t >= p["episode_length"]))
+            done=np.int32(self.done))
 
     def state(self):
         gs, t = self.gs, self.t
@@ -196,12 +207,13 @@ class CovidOracleEnv:
                     deaths=gs["Deaths"][t], vaccinated=gs["Vaccinated"][t], unemployed=gs["Unemployed"][t],
                     stringency=gs["Stringency Level"][t], subsidy=gs["Subsidy"][t],
                     postsubsidy=gs["Postsubsidy Productivity"][t], cooldown_until=self.cooldown_until.copy(),
-                    subsidy_level=int(self.subsidy_level), vaccines_available=self.vaccines_available.copy())
+                    subsidy_level=int(self.subsidy_level), vaccines_available=self.vaccines_available.copy(),
+                    episodes=self.episodes)
 
 
 class CovidOracleBatch:
-    def __init__(self, params, n_envs):
-        self.envs = [CovidOracleEnv(params) for _ in range(n_envs)]
+    def __init__(self, params, n_envs, auto_reset=False):
+        self.envs = [CovidOracleEnv(params, auto_reset) for _ in range(n_envs)]
 
     def step(self, act_a, act_p):
         for e, env in enumerate(self.envs):

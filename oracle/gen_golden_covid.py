@@ -1,6 +1,11 @@
 """TEST INFRASTRUCTURE: record a COVID-19 golden trace from the UNMODIFIED reference (build container only) and,
 with --check, step oracle/covid_oracle.py beside it.  Config = tests/run_covid19_cpu_gpu_consistency_checks.py:44-81.
 Usage: python oracle/gen_golden_covid.py [--check] [--steps N]
+       python oracle/gen_golden_covid.py --variant NAME [--check]     (one of VARIANTS, into tests/golden/covid_variants/)
+
+A variant trace runs across episode ends: the step that returns `done` records that step's rewards and `done`, then
+env.reset() and records the reset observation as that step's observation (what the product's auto-reset returns), and
+the trace goes on into the next episode: two full episodes and VARIANT_EXTRA_STEPS steps of the third.
 """
 import argparse
 import contextlib
@@ -15,8 +20,49 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import ref_harness as rh  # noqa: E402
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden_covid")
+VARIANT_OUT = os.path.join(os.path.dirname(OUT), "golden", "covid_variants")
 
 from ai_economist_b200.workloads import COVID_KWARGS, covid_reference_config  # noqa: E402
+
+# Parameter variants of the COVID workload: name -> (action seed, kwargs over COVID_KWARGS).  Each reaches device code
+# the default parameters do not:
+#   eta3_cooldown1_levels1      x ** -2 through the general powf; a 2-entry planner segment; vaccine deliveries that began
+#                               before the start date (every 7th day from day 7); change lists overflowing (cooldown 1)
+#   eta05_cooldown7_interval1   x ** 0.5 (the sqrt path); a planner mask open at every step
+#   eta15_levels40_health       x ** -0.5 through the general powf; a 41-entry planner segment (longer than a warp);
+#                               other health weights
+#   cooldown1_len60             the defaults with 1-day cooldowns: auto-reset of overflowed change lists
+#   early_start_daily_vaccines  the initial history window padded before the data begins; daily deliveries from day 10
+#   late_start_window_drops     the last start date with complete data: the real-world changes of the initial window reach its
+#                               oldest index and leave it (from step 121), so change-list entries drop off the front
+VARIANTS = {
+    "eta3_cooldown1_levels1": (21, dict(
+        episode_length=50, economic_reward_crra_eta=3.0, action_cooldown_period=1, subsidy_interval=30,
+        num_subsidy_levels=1, start_date="2020-10-15", vaccine_delivery_start_date="2020-07-01", delivery_interval=7,
+        daily_vaccines_per_million_people=10000)),
+    "eta05_cooldown7_interval1": (22, dict(
+        episode_length=40, economic_reward_crra_eta=0.5, action_cooldown_period=7, subsidy_interval=1,
+        num_subsidy_levels=5, start_date="2020-06-01")),
+    "eta15_levels40_health": (23, dict(
+        episode_length=70, economic_reward_crra_eta=1.5, action_cooldown_period=28, num_subsidy_levels=40,
+        subsidy_interval=30, health_priority_scaling_agents=1.0, health_priority_scaling_planner=2.0)),
+    "cooldown1_len60": (24, dict(episode_length=60, action_cooldown_period=1)),
+    "early_start_daily_vaccines": (25, dict(
+        episode_length=45, economic_reward_crra_eta=2, start_date="2020-03-22", daily_vaccines_per_million_people=10000,
+        delivery_interval=1, vaccine_delivery_start_date="2020-04-01", subsidy_interval=90)),
+    "late_start_window_drops": (26, dict(episode_length=130, start_date="2021-04-30", subsidy_interval=45)),
+}
+VARIANT_EXTRA_STEPS = 5
+
+
+def variant_kwargs(name):
+    """(full kwargs, action seed) of a named variant"""
+    seed, over = VARIANTS[name]
+    return dict(COVID_KWARGS, **over), seed
+
+
+def variant_path(name):
+    return os.path.join(VARIANT_OUT, "%s.npz" % name)
 
 
 def reference_config(kw):
@@ -66,11 +112,17 @@ def main():
     ap.add_argument("--cooldown", type=int, default=None, help="action_cooldown_period of the variant (default: the workload's 28)")
     ap.add_argument("--episode-length", type=int, default=None)
     ap.add_argument("--name", default=None, help="file name stem (default covid_seed<seed>)")
+    ap.add_argument("--variant", default=None, choices=sorted(VARIANTS),
+                    help="record the named variant across two episode ends (ignores --steps, --seed, --cooldown, --episode-length)")
     args = ap.parse_args()
     kwargs = dict(COVID_KWARGS)
-    if args.cooldown is not None:
+    multi_episode = args.variant is not None
+    if multi_episode:
+        kwargs, args.seed = variant_kwargs(args.variant)
+        args.steps = 2 * kwargs["episode_length"] + VARIANT_EXTRA_STEPS
+    if args.cooldown is not None and not multi_episode:
         kwargs["action_cooldown_period"] = args.cooldown
-    if args.episode_length is not None:
+    if args.episode_length is not None and not multi_episode:
         kwargs["episode_length"] = args.episode_length
         args.steps = min(args.steps, args.episode_length)
     f = rh.load_reference_foundation()
@@ -81,7 +133,7 @@ def main():
     if args.check:
         from ai_economist_b200.foundation.covid19 import build_covid_params
         from oracle.covid_oracle import CovidOracleEnv
-        orc = CovidOracleEnv(build_covid_params(**kwargs))
+        orc = CovidOracleEnv(build_covid_params(**kwargs), auto_reset=multi_episode)
     rng = np.random.RandomState(args.seed)
     rec = {k: [v] for k, v in ref_arrays(env, obs).items()}
     acts_a, acts_p = [], []
@@ -105,6 +157,9 @@ def main():
         actions["p"] = int(act_p)
         obs, rew, done, _ = env.step(actions)
         acts_a.append(act_a); acts_p.append(act_p)
+        if multi_episode and done["__all__"]:
+            with contextlib.redirect_stdout(io.StringIO()):
+                obs = env.reset()
         ra = ref_arrays(env, obs, rew, done)
         for k, v in ra.items():
             rec.setdefault(k, []).append(v)
@@ -113,8 +168,10 @@ def main():
             n_exact += check(t, ra)
     if orc:
         print("oracle matches the reference for %d steps (bit-exact float32 observations on %d of them)" % (args.steps, n_exact))
-    os.makedirs(OUT, exist_ok=True)
-    out = {"meta_json": np.array(json.dumps(dict(kwargs=kwargs, seed=args.seed, n_steps=args.steps)))}
+    meta = dict(kwargs=kwargs, seed=args.seed, n_steps=args.steps)
+    if multi_episode:
+        meta.update(variant=args.variant, reset_at_done=True)
+    out = {"meta_json": np.array(json.dumps(meta))}
     out["act_a"] = np.stack(acts_a).astype(np.int8)
     out["act_p"] = np.array(acts_p, np.int8)
     for k, v in rec.items():
@@ -122,7 +179,8 @@ def main():
             out[k] = np.stack(v)          # steps 1..N
         else:
             out[k] = np.stack(v)          # steps 0..N
-    path = os.path.join(OUT, "%s.npz" % (args.name or "covid_seed%d" % args.seed))
+    path = variant_path(args.variant) if multi_episode else os.path.join(OUT, "%s.npz" % (args.name or "covid_seed%d" % args.seed))
+    os.makedirs(os.path.dirname(path), exist_ok=True)
     np.savez_compressed(path, **out)
     print(path, "%.1f KB" % (os.path.getsize(path) / 1024))
 
