@@ -174,6 +174,13 @@ class AieCovidBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in _COVID_BUF_NAMES] + [("changes", C.c_void_p)]
 
 
+COVID_OBS_NAMES = _COVID_BUF_NAMES[6:13]   # the observation / mask tensors (aie_covid_obs_buffers)
+
+
+class AieCovidObsBuffers(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in COVID_OBS_NAMES]
+
+
 class AieError(RuntimeError):
     pass
 
@@ -237,11 +244,12 @@ def load_library(path=None):
     L.aie_covid_bind_buffers.argtypes = [P, C.POINTER(AieCovidBuffers)]
     L.aie_covid_reset.argtypes = [P, P]
     L.aie_covid_step.argtypes = [P, P]
+    L.aie_covid_step_final.argtypes = [P, C.POINTER(AieCovidObsBuffers), P]
     L.aie_covid_sample_random_actions.argtypes = [P, C.c_uint64, P]
     L.aie_covid_launch_count.argtypes = [P]
     L.aie_covid_launch_count.restype = C.c_int64
     for fn in ["aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
-               "aie_covid_sample_random_actions"]:
+               "aie_covid_step_final", "aie_covid_sample_random_actions"]:
         getattr(L, fn).restype = C.c_int
     L.aie_launch_count.restype = C.c_int64
     for fn in ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field", "aie_bind_buffers", "aie_load_state",
@@ -258,7 +266,7 @@ EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field"
                     "aie_set_fused_policy", "aie_sample_policy", "aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_compute_advantages", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
                     "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
-                    "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
+                    "aie_covid_step_final", "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
                     "aie_covid_evaluate_policy_backward", "aie_covid_compute_advantages", "aie_covid_launch_count"]
 
 

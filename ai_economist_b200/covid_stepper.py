@@ -71,7 +71,13 @@ def covid_config_from_params(p, auto_reset=True):
 class CovidStepperBase(PolicySampler):
     _DT = {"f32": np.float32, "f64": np.float64, "i32": np.int32, "i8": np.int8}
 
-    def __init__(self, params, n_envs, lib, device_index=0, auto_reset=True, change_list=None):
+    def __init__(self, params, n_envs, lib, device_index=0, auto_reset=True, change_list=None, final_obs=False):
+        # final_obs: keep final_<name> twins of the seven observation / mask buffers; step() then writes into row e the
+        # observations of the state replica e's episode ended in, when that step ends it (done == 1).  Needs auto_reset.
+        if final_obs and not auto_reset:
+            raise ValueError("final_obs=True needs auto_reset=True: without the auto-reset, the observations after the step "
+                             "that ends an episode already are its final ones")
+        self.final_obs = bool(final_obs)
         # change_list: keep a persistent per-state list of stringency changes (O(changes) unemployment response instead
         # of a history scan, whose cost grows with the episode).  Default ON; AIE_COVID_CHANGE_LIST=0 selects the scan.
         if change_list is None:
@@ -103,6 +109,11 @@ class CovidStepperBase(PolicySampler):
             setattr(bufs, name, self._ptr(self.buf[name]))
         bufs.changes = self._ptr(self.buf["changes"]) if self.change_list else None
         self._check(lib.aie_covid_bind_buffers(self._h, C.byref(bufs)))
+        if self.final_obs:
+            self._final_bufs = _abi.AieCovidObsBuffers()
+            for name in _abi.COVID_OBS_NAMES:
+                self.buf["final_" + name] = self._alloc(shapes[name][1], shapes[name][0])
+                setattr(self._final_bufs, name, self._ptr(self.buf["final_" + name]))
 
     def _check(self, rc):
         if rc != _abi.AIE_OK:
@@ -126,7 +137,10 @@ class CovidStepperBase(PolicySampler):
         self._check(self.lib.aie_covid_reset(self._h, self._stream()))
 
     def step(self):
-        self._check(self.lib.aie_covid_step(self._h, self._stream()))
+        if self.final_obs:
+            self._check(self.lib.aie_covid_step_final(self._h, C.byref(self._final_bufs), self._stream()))
+        else:
+            self._check(self.lib.aie_covid_step(self._h, self._stream()))
 
     def sample_random_actions(self, seed=0):
         self._check(self.lib.aie_covid_sample_random_actions(self._h, C.c_uint64(int(seed)), self._stream()))
@@ -173,7 +187,7 @@ class CovidStepperBase(PolicySampler):
 
 
 class CudaCovidStepper(CovidStepperBase):
-    def __init__(self, params, n_envs, device="cuda:0", auto_reset=True, lib_path=None, change_list=None):
+    def __init__(self, params, n_envs, device="cuda:0", auto_reset=True, lib_path=None, change_list=None, final_obs=False):
         import torch
 
         if not torch.cuda.is_available():
@@ -184,7 +198,8 @@ class CudaCovidStepper(CovidStepperBase):
         self.device = torch.device("cuda", idx)
         lib = _abi.load_library(lib_path)
         with torch.cuda.device(self.device):
-            super().__init__(params, n_envs, lib, device_index=idx, auto_reset=auto_reset, change_list=change_list)
+            super().__init__(params, n_envs, lib, device_index=idx, auto_reset=auto_reset, change_list=change_list,
+                             final_obs=final_obs)
 
     def _alloc(self, shape, dt):
         t = self.torch

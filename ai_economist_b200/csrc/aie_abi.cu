@@ -22,6 +22,9 @@
 //                          (aie_evaluate_policy_backward); instantiated for float32 / bfloat16 masks and logits.
 //   aie_covid_evaluate_policy_kernel, aie_covid_evaluate_policy_backward_kernel  one warp per (row, state | planner):
 //                          the same for the COVID-19 scenario.
+//   aie_covid_step_final_kernel  aie_covid_step_kernel's launch shape and body; on the step that ends an episode it
+//                          also writes the observations of the state the episode ended in into the caller's tensors,
+//                          before the auto-reset overwrites that state (aie_covid_step_final).
 //   aie_compute_advantages_kernel  one thread per column of a stored rollout (agent and planner columns, group-uniform
 //                          CTAs): advantages and value targets (aie_compute_advantages, aie_covid_compute_advantages).
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
@@ -107,6 +110,7 @@ void *dev_alloc(size_t bytes);
 void const_free(void *dev);
 int covid_launch_reset(aie_covid_env *, void *stream);
 int covid_launch_step(aie_covid_env *, void *stream);
+int covid_launch_step_final(aie_covid_env *, const CovidBufs &fin, void *stream);
 int covid_launch_sample(aie_covid_env *, uint64_t key, void *stream);
 int covid_launch_policy(aie_covid_env *, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream);
 int launch_policy_eval(aie_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows, void *stream);
@@ -1004,6 +1008,13 @@ __global__ void __launch_bounds__(64) aie_covid_step_kernel(const __grid_constan
     __shared__ uint32_t chg[64 * CV_CHG_CAP];
     covid_step_env(c, blockIdx.x, b, red, chg, threadIdx.x, blockDim.x);
 }
+// aie_covid_step_final: the same step; the step that ends an episode also writes its final observations into fin.
+__global__ void __launch_bounds__(64) aie_covid_step_final_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                  const CovidBufs fin) {
+    __shared__ float red[3 * 64];
+    __shared__ uint32_t chg[64 * CV_CHG_CAP];
+    covid_step_env<true>(c, blockIdx.x, b, fin, red, chg, threadIdx.x, blockDim.x);
+}
 __global__ void __launch_bounds__(64) aie_covid_reset_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b) {
     covid_reset_env(c, blockIdx.x, b, threadIdx.x, blockDim.x, false);
 }
@@ -1097,6 +1108,12 @@ int covid_launch_policy_eval(aie_covid_env *env, const PolicyEvalBufs &p, int mt
 int covid_launch_step(aie_covid_env *env, void *stream) {
     aie_covid_step_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     AIE_CUDA(cudaGetLastError(), "aie_covid_step_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+int covid_launch_step_final(aie_covid_env *env, const CovidBufs &fin, void *stream) {
+    aie_covid_step_final_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, fin);
+    AIE_CUDA(cudaGetLastError(), "aie_covid_step_final_kernel launch");
     env->launches++;
     return AIE_OK;
 }

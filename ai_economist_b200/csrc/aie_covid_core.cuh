@@ -201,7 +201,12 @@ CV_DEV double cv_accumulate_changes(const CovidCfg &c, const uint32_t *lst, int 
 // chg: scratch uint32 [nthr][CV_CHG_CAP] (shared memory on the device): per-state list of the stringency changes in
 // the history window
 constexpr int CV_CHG_CAP = 32;
-CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, float *red, uint32_t *chg, int tid, int nthr) {
+// FINAL: on the step that ends an episode under the auto-reset, first write the observations / masks of the state the
+// episode ended in into row e of fin's seven observation / mask tensors (fin: b with those pointers replaced), then
+// reset.  Unused without FINAL.
+template <bool FINAL>
+CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const CovidBufs &fin, float *red, uint32_t *chg,
+                           int tid, int nthr) {
     const int S = c.S, L = c.L, L1 = c.L + 1, F = c.F;
     float *st = b.state + (size_t)e * CVS_FIELDS * S;
     int32_t *ints = b.ints + (size_t)e * 2 * S;
@@ -383,8 +388,22 @@ CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, float *
         hdr[CVH_T] = t; hdr[CVH_SUBSIDY_LEVEL] = level; hdr[CVH_RING_HEAD] = new_head;
     }
     cv_bsync();
-    if (c.auto_reset && t >= c.T) covid_reset_env(c, e, b, tid, nthr, true);
+    if (FINAL) {
+        // One observation pass whose destination is chosen per step: a second inlined pass for the ending step made
+        // the ordinary steps of this kernel 7.7 % slower on an H100 (the code ptxas makes of the whole body); this form
+        // leaves them unchanged (DESIGN §6).
+        const bool end = c.auto_reset && t >= c.T;
+        covid_observe(c, st, ints, hdr, ring, new_head, e, end ? fin : b, tid, nthr);
+        if (end) {
+            cv_bsync();   // once per episode: the reset below overwrites what the final pass reads
+            covid_reset_env(c, e, b, tid, nthr, true);
+        }
+    } else if (c.auto_reset && t >= c.T) covid_reset_env(c, e, b, tid, nthr, true);
     else covid_observe(c, st, ints, hdr, ring, new_head, e, b, tid, nthr);
+}
+// The step without final observations (aie_covid_step).
+CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, float *red, uint32_t *chg, int tid, int nthr) {
+    covid_step_env<false>(c, e, b, b, red, chg, tid, nthr);
 }
 
 // Random policy: uniform over the unmasked actions (NO-OP is always open).

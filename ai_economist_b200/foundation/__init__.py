@@ -17,7 +17,7 @@ scenarios = _scenarios_mod.scenario_registry
 
 def make_env_instance(scenario_name, **kwargs):
     """Same call as the reference; extra kwargs: n_envs (default 1), device ("cuda:0"), seeds, auto_reset, obs_dtype,
-    final_obs (BatchedFoundationEnv), and
+    final_obs, and
     reference_api (or AIE_REFERENCE_API=1 in the environment): wrap replica 0 in adapters.ReferenceApiEnv, whose
     reset()/step() take and return the reference's nested numpy dictionaries, so tutorial code runs unchanged."""
     import os

@@ -225,8 +225,9 @@ class CovidBatchedEnv:
         from .._abi import obs_dtype_name
         if obs_dtype_name(obs_dtype) != "float32":
             raise NotImplementedError("the COVID-19 scenario writes float32 observations only")
-        if final_obs:
-            raise NotImplementedError("final_obs is not available for the COVID-19 scenario")
+        if final_obs and not auto_reset:
+            raise ValueError("final_obs=True needs auto_reset=True: without the auto-reset, env.obs after the step that "
+                             "ends an episode already is its final observation")
         assert collate_agent_step_and_reset_data, \
             "The env. config 'collate_agent_step_and_reset_data' should be set to True."
         if use_real_world_data or use_real_world_policies:
@@ -259,9 +260,16 @@ class CovidBatchedEnv:
         self._episode_length = int(episode_length)
         if stepper_factory is None:
             from ..covid_stepper import CudaCovidStepper
-            self._stepper = CudaCovidStepper(self.params, self.n_envs, device=device, auto_reset=auto_reset)
+            self._stepper = CudaCovidStepper(self.params, self.n_envs, device=device, auto_reset=auto_reset,
+                                             final_obs=bool(final_obs))
+        elif final_obs:
+            self._stepper = stepper_factory(self.params, self.n_envs, auto_reset, final_obs=True)
+            if not getattr(self._stepper, "final_obs", False):
+                raise NotImplementedError("final_obs=True: the stepper made by stepper_factory does not write final "
+                                          "observations (it needs final_<name> buffers and a final-observation step)")
         else:
             self._stepper = stepper_factory(self.params, self.n_envs, auto_reset)
+        self._final_obs = bool(final_obs)
         self._loaded = False
         self._build_views()
         self._build_rate_observation()
@@ -305,32 +313,42 @@ class CovidBatchedEnv:
     def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0):
         """Advantages and value targets of a stored rollout (the contract of BatchedFoundationEnv.compute_advantages),
         A = 51 states: rewards = (rew["a"] [T, E, 51] float32, rew["p"] [T, E] float64) stacked over the steps, values
-        = (agent, planner) float32 of the same shapes, dones int32 [T, E], last_values = ([E, 51], [E]).  This env has
-        no final observations yet, so final_values is normally None: an episode end is then treated as terminal."""
+        = (agent, planner) float32 of the same shapes, dones int32 [T, E], last_values = ([E, 51], [E]).  Every episode
+        ends on its time limit, so it is truncated: final_values = the values of env.final_obs stored at each step
+        (env created with final_obs=True) bootstraps it; final_values=None treats an episode end as terminal."""
         return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam)
 
     def _build_views(self):
         b = self._stepper.buf
-        S = self.n_agents
-        sc = b["obs_scalars"]
-        exp = (lambda v: v[:, None].expand(-1, S)) if hasattr(sc, "expand") else (lambda v: np.repeat(v[:, None], S, axis=1))
-        self.obs = {
-            "a": {"world-agent_state": b["obs_agent_state"], "world-agent_postsubsidy_productivity": b["obs_postsubsidy"],
-                  "world-lagged_stringency_level": b["obs_lagged_stringency"], "time": exp(sc[:, 0]),
-                  "ControlUSStateOpenCloseStatus-agent_policy_indicators": b["obs_policy_indicators"],
-                  "FederalGovernmentSubsidy-t_until_next_subsidy": exp(sc[:, 1]),
-                  "FederalGovernmentSubsidy-current_subsidy_level": exp(sc[:, 2]),
-                  "VaccinationCampaign-t_until_next_vaccines": exp(sc[:, 3]), "action_mask": b["mask_agent"]},
-            "p": {"world-agent_state": b["obs_agent_state"], "world-agent_postsubsidy_productivity": b["obs_postsubsidy"],
-                  "world-lagged_stringency_level": b["obs_lagged_stringency"], "time": sc[:, 0:1],
-                  "ControlUSStateOpenCloseStatus-agent_policy_indicators": b["obs_policy_indicators"],
-                  "FederalGovernmentSubsidy-t_until_next_subsidy": sc[:, 1],
-                  "FederalGovernmentSubsidy-current_subsidy_level": sc[:, 2],
-                  "VaccinationCampaign-t_until_next_vaccines": sc[:, 3], "action_mask": b["mask_planner"]},
-        }
+        self.obs = self._obs_views(b, "")
+        # final_obs=True: env.final_obs mirrors env.obs over the final_<name> buffers.  After a step, row e of a replica
+        # with done["__all__"][e] == 1 holds the observation of the state its episode ended in (env.obs already shows the
+        # next episode's first); the other rows keep whatever an earlier episode end wrote.  reset() does not touch them.
+        self.final_obs = self._obs_views(b, "final_") if self._final_obs else None
         self.rew = {"a": b["reward_agent"], "p": b["reward_planner"]}
         self.done = {"__all__": b["done"]}
         self.info = {"a": {}, "p": {}}
+
+    def _obs_views(self, b, prefix):
+        """The collated "a" / "p" observation dict over the observation / mask buffers b[prefix + name]."""
+        g = lambda k: b[prefix + k]
+        S = self.n_agents
+        sc = g("obs_scalars")
+        exp = (lambda v: v[:, None].expand(-1, S)) if hasattr(sc, "expand") else (lambda v: np.repeat(v[:, None], S, axis=1))
+        return {
+            "a": {"world-agent_state": g("obs_agent_state"), "world-agent_postsubsidy_productivity": g("obs_postsubsidy"),
+                  "world-lagged_stringency_level": g("obs_lagged_stringency"), "time": exp(sc[:, 0]),
+                  "ControlUSStateOpenCloseStatus-agent_policy_indicators": g("obs_policy_indicators"),
+                  "FederalGovernmentSubsidy-t_until_next_subsidy": exp(sc[:, 1]),
+                  "FederalGovernmentSubsidy-current_subsidy_level": exp(sc[:, 2]),
+                  "VaccinationCampaign-t_until_next_vaccines": exp(sc[:, 3]), "action_mask": g("mask_agent")},
+            "p": {"world-agent_state": g("obs_agent_state"), "world-agent_postsubsidy_productivity": g("obs_postsubsidy"),
+                  "world-lagged_stringency_level": g("obs_lagged_stringency"), "time": sc[:, 0:1],
+                  "ControlUSStateOpenCloseStatus-agent_policy_indicators": g("obs_policy_indicators"),
+                  "FederalGovernmentSubsidy-t_until_next_subsidy": sc[:, 1],
+                  "FederalGovernmentSubsidy-current_subsidy_level": sc[:, 2],
+                  "VaccinationCampaign-t_until_next_vaccines": sc[:, 3], "action_mask": g("mask_planner")},
+        }
 
     def _build_rate_observation(self):
         """VaccinationCampaign(observe_rate=True) (covid19_components.py:629-661): the vaccination rate of the NEXT timestep, 0
@@ -353,21 +371,45 @@ class CovidBatchedEnv:
             self._rate_a, self._rate_p = torch.zeros((E, S), dtype=torch.float32, device=sc.device), torch.zeros(E, dtype=torch.float32, device=sc.device)
         self.obs["a"]["VaccinationCampaign-next_vaccination_rate"] = self._rate_a
         self.obs["p"]["VaccinationCampaign-next_vaccination_rate"] = self._rate_p
+        if self.final_obs is not None:
+            if isinstance(sc, np.ndarray):
+                self._final_rate_a, self._final_rate_p = np.zeros_like(self._rate_a), np.zeros_like(self._rate_p)
+            else:
+                self._final_rate_a, self._final_rate_p = torch.zeros_like(self._rate_a), torch.zeros_like(self._rate_p)
+            self.final_obs["a"]["VaccinationCampaign-next_vaccination_rate"] = self._final_rate_a
+            self.final_obs["p"]["VaccinationCampaign-next_vaccination_rate"] = self._final_rate_p
 
-    def _refresh_rate_observation(self):
-        if self._rate_tab is None:
-            return
-        sc = self._stepper.buf["obs_scalars"]   # [:, 0] = timestep / time_scale (episode_length under observation scaling)
+    def _rate_of(self, sc):
+        """The table's rate at the timesteps of obs_scalars sc: [:, 0] = timestep / time_scale (episode_length under
+        observation scaling)."""
         scale = float(self.params["time_scale"])
         if isinstance(sc, np.ndarray):
-            t = np.rint(sc[:, 0].astype(np.float64) * scale).astype(np.int64)
-            self._rate_p[...] = self._rate_tab[t]
+            return self._rate_tab[np.rint(sc[:, 0].astype(np.float64) * scale).astype(np.int64)]
+        import torch
+        return self._rate_tab[torch.round(sc[:, 0].double() * scale).long()]
+
+    def _refresh_rate_observation(self, stepped=False):
+        if self._rate_tab is None:
+            return
+        b = self._stepper.buf
+        rate = self._rate_of(b["obs_scalars"])
+        if isinstance(rate, np.ndarray):
+            self._rate_p[...] = rate
             self._rate_a[...] = self._rate_p[:, None]
         else:
-            import torch
-            t = torch.round(sc[:, 0].double() * scale).long()
-            self._rate_p.copy_(self._rate_tab[t])
+            self._rate_p.copy_(rate)
             self._rate_a.copy_(self._rate_p[:, None].expand_as(self._rate_a))
+        if stepped and self.final_obs is not None:
+            # only the rows of the episodes this step ended: their own time scalar is t = T (the table's last entry)
+            done = b["done"] != 0
+            rate = self._rate_of(b["final_obs_scalars"])
+            if isinstance(rate, np.ndarray):
+                self._final_rate_p[...] = np.where(done, rate, self._final_rate_p)
+                self._final_rate_a[...] = np.where(done[:, None], rate[:, None], self._final_rate_a)
+            else:
+                import torch
+                self._final_rate_p.copy_(torch.where(done, rate, self._final_rate_p))
+                self._final_rate_a.copy_(torch.where(done[:, None], rate[:, None], self._final_rate_a))
 
     def reset(self):
         self._stepper.reset()
@@ -395,7 +437,7 @@ class CovidBatchedEnv:
                         buf[...] = torch.as_tensor(np.asarray(v) if not isinstance(v, torch.Tensor) else v,
                                                    device=buf.device).to(buf.dtype).reshape(buf.shape)
         self._stepper.step()
-        self._refresh_rate_observation()
+        self._refresh_rate_observation(stepped=True)
         return self.obs, self.rew, self.done, self.info
 
 

@@ -635,6 +635,20 @@ int aie_covid_bind_buffers(aie_covid_env *env, const aie_covid_buffers *bufs);
 int aie_covid_reset(aie_covid_env *env, void *stream);
 /* One env.step() for every replica: 3 component steps + scenario step + observations + rewards + done. */
 int aie_covid_step(aie_covid_env *env, void *stream);
+
+/* The seven observation / mask tensors of aie_covid_buffers, with the same shapes, float32. */
+typedef struct aie_covid_obs_buffers {
+    float *obs_agent_state, *obs_postsubsidy, *obs_lagged_stringency, *obs_policy_indicators, *obs_scalars,
+          *mask_agent, *mask_planner;
+} aie_covid_obs_buffers;
+
+/* ABI 5.  aie_covid_step, and in the same launch the final observations of the episodes it ends: for every env whose
+ * done flag this step sets, row e of `final_out` receives what aie_covid_step writes for that env with auto_reset off
+ * (the observations and masks of the state its episode ended in; the bound tensors already show the next episode's
+ * first).  Rows of the other envs are left untouched.  What a trainer bootstraps a truncated episode's value from.
+ * One launch, asynchronous on `stream`.  AIE_EINVAL for a NULL env or final_out, a NULL member or a member not 4-byte
+ * aligned; AIE_ESTATE before buffers are bound and the env has been reset, or with auto_reset off. */
+int aie_covid_step_final(aie_covid_env *env, const aie_covid_obs_buffers *final_out, void *stream);
 /* Random policy on the device (uniform over the unmasked actions of the current masks); see aie_sample_random_actions. */
 int aie_covid_sample_random_actions(aie_covid_env *env, uint64_t seed, void *stream);
 /* A policy's actions on the device (the contract of aie_sample_policy): agent logits [E, S, 1 + levels] (action axis
