@@ -4,10 +4,10 @@ import ctypes as C
 import numpy as np
 import os
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 MAX_COMPONENTS, MAX_BRACKETS, MAX_RATES = 8, 16, 64
 AIE_OK = 0
-OBS_F32, OBS_BF16 = 0, 1   # aie_config.obs_dtype
+OBS_F32, OBS_BF16 = 0, 1   # aie_config.obs_dtype, aie_covid_config.obs_dtype
 REWARD_F32, REWARD_F64 = 0, 1   # aie_advantage_args.rewards_*_dtype
 
 COMPONENT_KIND = {"Build": 0, "ContinuousDoubleAuction": 1, "Gather": 2, "PeriodicBracketTax": 3,
@@ -162,7 +162,8 @@ class AieCovidConfig(C.Structure):
             "daily_production_per_worker", "maximum_productivity", "agents_health_norm", "agents_economic_norm",
             "min_agent_health", "max_agent_health", "min_agent_econ", "max_agent_econ", "w_agent_health",
             "w_agent_econ", "conv_weights", "conv_filters", "max_daily_subsidy_per_state", "rw_policy",
-            "init_state"]])
+            "init_state"]]
+        + [("obs_dtype", C.c_int32)])
 
 
 _COVID_BUF_NAMES = ["state", "ints", "hdr", "ring", "actions_agent", "actions_planner", "obs_agent_state",

@@ -4,13 +4,14 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from .stepper import PolicySampler, buf_kind_torch, float_kind_torch, is_i32_torch
+from .stepper import PolicySampler, bf16_bits_to_float32, buf_kind_torch, float_kind_torch, is_i32_torch
 
 F32, I32 = np.float32, np.int32
 
 
-def covid_config_from_params(p, auto_reset=True):
-    """p: dict from foundation.covid19.build_covid_params.  Returns (AieCovidConfig, keep-alive list)."""
+def covid_config_from_params(p, auto_reset=True, obs_dtype=None):
+    """p: dict from foundation.covid19.build_covid_params; obs_dtype: the observations' element type (torch.float32 /
+    torch.bfloat16 or their names, None: float32).  Returns (AieCovidConfig, keep-alive list)."""
     cfg = _abi.AieCovidConfig()
     keep = []
 
@@ -36,6 +37,7 @@ def covid_config_from_params(p, auto_reset=True):
     cfg.rw_policy_days = int(p["rw_policy"].shape[0])
     cfg.value_of_life = int(p["value_of_life"])
     cfg.auto_reset = int(bool(auto_reset))
+    cfg.obs_dtype = {"float32": _abi.OBS_F32, "bfloat16": _abi.OBS_BF16}[_abi.obs_dtype_name(obs_dtype)]
     for dst, src in [("gamma", "gamma"), ("death_rate", "death_rate"),
                      ("infection_too_sick_to_work_rate", "infection_too_sick_to_work_rate"),
                      ("pop_between_age_18_65", "pop_between_age_18_65"), ("risk_free_interest_rate", "risk_free_interest_rate"),
@@ -69,9 +71,14 @@ def covid_config_from_params(p, auto_reset=True):
 
 
 class CovidStepperBase(PolicySampler):
-    _DT = {"f32": np.float32, "f64": np.float64, "i32": np.int32, "i8": np.int8}
+    # "bf16": the observation / mask buffers of a bfloat16 env; numpy backends hold their raw bits
+    _DT = {"f32": np.float32, "f64": np.float64, "i32": np.int32, "i8": np.int8, "bf16": np.uint16}
 
-    def __init__(self, params, n_envs, lib, device_index=0, auto_reset=True, change_list=None, final_obs=False):
+    def __init__(self, params, n_envs, lib, device_index=0, auto_reset=True, change_list=None, final_obs=False,
+                 obs_dtype=None):
+        # obs_dtype: element type of the seven observation / mask buffers (and their final_ twins), float32 (default)
+        # or bfloat16, each element the round-to-nearest-even of the float32 a float32 env writes.
+        self.obs_dtype = _abi.obs_dtype_name(obs_dtype)
         # final_obs: keep final_<name> twins of the seven observation / mask buffers; step() then writes into row e the
         # observations of the state replica e's episode ended in, when that step ends it (done == 1).  Needs auto_reset.
         if final_obs and not auto_reset:
@@ -87,18 +94,19 @@ class CovidStepperBase(PolicySampler):
         self.p = params
         self.n_envs = int(n_envs)
         self.lib = lib
-        cfg, self._keep = covid_config_from_params(params, auto_reset)
+        cfg, self._keep = covid_config_from_params(params, auto_reset, self.obs_dtype)
         h = C.c_void_p()
         self._check(lib.aie_covid_create(C.byref(cfg), self.n_envs, int(device_index), C.byref(h)))
         self._h = h
         E, S, L = self.n_envs, params["n_states"], params["filter_len"]
+        fo = "bf16" if self.obs_dtype == "bfloat16" else "f32"   # the observation / mask tensors
         shapes = {
             "state": ("f32", (E, 9, S)), "ints": ("i32", (E, 2, S)), "hdr": ("i32", (E, 4)), "ring": ("i8", (E, S, (L + 1 + 15) // 16 * 16)),
             "actions_agent": ("i32", (E, S)), "actions_planner": ("i32", (E,)),
-            "obs_agent_state": ("f32", (E, 6, S)), "obs_postsubsidy": ("f32", (E, S)),
-            "obs_lagged_stringency": ("f32", (E, S)), "obs_policy_indicators": ("f32", (E, S)),
-            "obs_scalars": ("f32", (E, 4)), "mask_agent": ("f32", (E, 1 + params["num_stringency_levels"], S)),
-            "mask_planner": ("f32", (E, 1 + params["num_subsidy_levels"])), "reward_agent": ("f32", (E, S)),
+            "obs_agent_state": (fo, (E, 6, S)), "obs_postsubsidy": (fo, (E, S)),
+            "obs_lagged_stringency": (fo, (E, S)), "obs_policy_indicators": (fo, (E, S)),
+            "obs_scalars": (fo, (E, 4)), "mask_agent": (fo, (E, 1 + params["num_stringency_levels"], S)),
+            "mask_planner": (fo, (E, 1 + params["num_subsidy_levels"])), "reward_agent": ("f32", (E, S)),
             "reward_planner": ("f64", (E,)), "done": ("i32", (E,)),
         }
         if self.change_list:
@@ -170,9 +178,14 @@ class CovidStepperBase(PolicySampler):
     def launch_count(self):
         return int(self.lib.aie_covid_launch_count(self._h))
 
+    def obs_to_numpy(self, name, e=None):
+        """Host copy of buffer `name` (of env e), bfloat16 observations as float32 (exact: every bfloat16 is a float32)."""
+        a = self.to_numpy(self.buf[name] if e is None else self.buf[name][e])
+        return bf16_bits_to_float32(a) if np.asarray(a).dtype == np.uint16 else a
+
     def read_obs(self, e):
-        """Host copy of env e's outputs in oracle/covid_oracle.py's layout."""
-        g = lambda k: self.to_numpy(self.buf[k][e])
+        """Host copy of env e's outputs in oracle/covid_oracle.py's layout (observations as float32)."""
+        g = lambda k: self.obs_to_numpy(k, e)
         return dict(agent_state=g("obs_agent_state"), postsubsidy=g("obs_postsubsidy"), lagged=g("obs_lagged_stringency"),
                     policy_ind=g("obs_policy_indicators"), scalars=g("obs_scalars"), mask_a=g("mask_agent"),
                     mask_p=g("mask_planner"), rew_a=g("reward_agent"), rew_p=np.float64(g("reward_planner")),
@@ -187,7 +200,8 @@ class CovidStepperBase(PolicySampler):
 
 
 class CudaCovidStepper(CovidStepperBase):
-    def __init__(self, params, n_envs, device="cuda:0", auto_reset=True, lib_path=None, change_list=None, final_obs=False):
+    def __init__(self, params, n_envs, device="cuda:0", auto_reset=True, lib_path=None, change_list=None, final_obs=False,
+                 obs_dtype=None):
         import torch
 
         if not torch.cuda.is_available():
@@ -199,11 +213,11 @@ class CudaCovidStepper(CovidStepperBase):
         lib = _abi.load_library(lib_path)
         with torch.cuda.device(self.device):
             super().__init__(params, n_envs, lib, device_index=idx, auto_reset=auto_reset, change_list=change_list,
-                             final_obs=final_obs)
+                             final_obs=final_obs, obs_dtype=obs_dtype)
 
     def _alloc(self, shape, dt):
         t = self.torch
-        m = {"i8": t.int8, "i32": t.int32, "f32": t.float32, "f64": t.float64}
+        m = {"i8": t.int8, "i32": t.int32, "f32": t.float32, "f64": t.float64, "bf16": t.bfloat16}
         return t.zeros(shape, dtype=m[dt], device=self.device)
 
     def _buf_kind(self, buf):
@@ -226,4 +240,6 @@ class CudaCovidStepper(CovidStepperBase):
         return C.c_void_p(self.torch.cuda.current_stream(self.device).cuda_stream)
 
     def to_numpy(self, buf):
+        if buf.dtype == self.torch.bfloat16:   # numpy has no bfloat16: float32 holds every value exactly
+            buf = buf.float()
         return buf.detach().cpu().numpy()

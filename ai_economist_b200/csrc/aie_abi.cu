@@ -25,6 +25,9 @@
 //   aie_covid_step_final_kernel  aie_covid_step_kernel's launch shape and body; on the step that ends an episode it
 //                          also writes the observations of the state the episode ended in into the caller's tensors,
 //                          before the auto-reset overwrites that state (aie_covid_step_final).
+//   aie_covid_{reset,step,step_final,sample}_bf16_kernel, aie_covid_sample_policy_kernel<LT, bf16_t>  the COVID-19
+//                          kernels over bfloat16 observations and masks (aie_covid_config::obs_dtype == AIE_OBS_BF16),
+//                          with their float32 twins' launch shapes.
 //   aie_compute_advantages_kernel  one thread per column of a stored rollout (agent and planner columns, group-uniform
 //                          CTAs): advantages and value targets (aie_compute_advantages, aie_covid_compute_advantages).
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
@@ -1022,15 +1025,45 @@ __global__ void __launch_bounds__(64) aie_covid_reset_kernel(const __grid_consta
 __global__ void __launch_bounds__(64) aie_covid_sample_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b, uint64_t key) {
     covid_sample_env(c, blockIdx.x, b, cv_mix64(key ^ cv_mix64(blockIdx.x)), threadIdx.x, blockDim.x);
 }
+// *_bf16: the same bodies over bfloat16 observation / mask tensors (aie_covid_config::obs_dtype == AIE_OBS_BF16), with
+// their float32 twins' launch shapes.
+__global__ void __launch_bounds__(64) aie_covid_step_bf16_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b) {
+    __shared__ float red[3 * 64];
+    __shared__ uint32_t chg[64 * CV_CHG_CAP];
+    covid_step_env<false, bf16_t>(c, blockIdx.x, b, b, red, chg, threadIdx.x, blockDim.x);
+}
+__global__ void __launch_bounds__(64) aie_covid_step_final_bf16_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                       const CovidBufs fin) {
+    __shared__ float red[3 * 64];
+    __shared__ uint32_t chg[64 * CV_CHG_CAP];
+    covid_step_env<true, bf16_t>(c, blockIdx.x, b, fin, red, chg, threadIdx.x, blockDim.x);
+}
+__global__ void __launch_bounds__(64) aie_covid_reset_bf16_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b) {
+    covid_reset_env<bf16_t>(c, blockIdx.x, b, threadIdx.x, blockDim.x, false);
+}
+__global__ void __launch_bounds__(64) aie_covid_sample_bf16_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                   uint64_t key) {
+    covid_sample_env<bf16_t>(c, blockIdx.x, b, cv_mix64(key ^ cv_mix64(blockIdx.x)), threadIdx.x, blockDim.x);
+}
 // Policy sampler (aie_covid_sample_policy): one warp per (env, unit), units = S states + the planner, eight per CTA.
-template <typename LT>
-__global__ void __launch_bounds__(256) aie_covid_sample_policy_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
-                                                                      const PolicyBufs p, uint64_t sd) {
+// LT: the logits' element type; MT: the masks' (bf16_t for a bfloat16 env).
+template <typename LT, typename MT>
+__device__ __forceinline__ void covid_sample_policy_body(const CovidCfg &c, const CovidBufs &b, const PolicyBufs &p, uint64_t sd) {
     const long long wid = (long long)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
     const int units = c.S + 1;
     const int env = (int)(wid / units), u = (int)(wid - (long long)env * units);
     if (env >= c.n_envs) return;
-    covid_policy_unit<LT>(c, env, b, p, cv_mix64(sd ^ cv_mix64((uint64_t)env)), u, threadIdx.x & 31);
+    covid_policy_unit<LT, MT>(c, env, b, p, cv_mix64(sd ^ cv_mix64((uint64_t)env)), u, threadIdx.x & 31);
+}
+template <typename LT>   // float32 masks
+__global__ void __launch_bounds__(256) aie_covid_sample_policy_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                      const PolicyBufs p, uint64_t sd) {
+    covid_sample_policy_body<LT, float>(c, b, p, sd);
+}
+template <typename LT, typename MT>
+__global__ void __launch_bounds__(256) aie_covid_sample_policy_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                      const PolicyBufs p, uint64_t sd) {
+    covid_sample_policy_body<LT, MT>(c, b, p, sd);
 }
 
 // Evaluation of stored actions (aie_covid_evaluate_policy, *_backward): one warp per (row, unit), units = S + 1.
@@ -1068,21 +1101,27 @@ void *dev_alloc(size_t bytes) {
 }
 void const_free(void *dev) { cudaFree(dev); }
 int covid_launch_reset(aie_covid_env *env, void *stream) {
-    aie_covid_reset_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
+    if (env->obs_bf16) aie_covid_reset_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
+    else aie_covid_reset_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     AIE_CUDA(cudaGetLastError(), "aie_covid_reset_kernel launch");
     env->launches++;
     return AIE_OK;
 }
 int covid_launch_sample(aie_covid_env *env, uint64_t key, void *stream) {
-    aie_covid_sample_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, key);
+    if (env->obs_bf16) aie_covid_sample_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, key);
+    else aie_covid_sample_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, key);
     AIE_CUDA(cudaGetLastError(), "aie_covid_sample_kernel launch");
     env->launches++;
     return AIE_OK;
 }
 int covid_launch_policy(aie_covid_env *env, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream) {
     const unsigned grid = (unsigned)(((long long)env->n_envs * (env->cfg.S + 1) + 7) / 8);
-    if (lt_bf16) aie_covid_sample_policy_kernel<bf16_t><<<grid, 256, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, p, sd);
-    else aie_covid_sample_policy_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, p, sd);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (env->obs_bf16) {
+        if (lt_bf16) aie_covid_sample_policy_kernel<bf16_t, bf16_t><<<grid, 256, 0, st>>>(env->cfg, env->bufs, p, sd);
+        else aie_covid_sample_policy_kernel<float, bf16_t><<<grid, 256, 0, st>>>(env->cfg, env->bufs, p, sd);
+    } else if (lt_bf16) aie_covid_sample_policy_kernel<bf16_t><<<grid, 256, 0, st>>>(env->cfg, env->bufs, p, sd);
+    else aie_covid_sample_policy_kernel<float><<<grid, 256, 0, st>>>(env->cfg, env->bufs, p, sd);
     AIE_CUDA(cudaGetLastError(), "aie_covid_sample_policy_kernel launch");
     env->launches++;
     return AIE_OK;
@@ -1106,13 +1145,15 @@ int covid_launch_policy_eval(aie_covid_env *env, const PolicyEvalBufs &p, int mt
     return AIE_OK;
 }
 int covid_launch_step(aie_covid_env *env, void *stream) {
-    aie_covid_step_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
+    if (env->obs_bf16) aie_covid_step_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
+    else aie_covid_step_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     AIE_CUDA(cudaGetLastError(), "aie_covid_step_kernel launch");
     env->launches++;
     return AIE_OK;
 }
 int covid_launch_step_final(aie_covid_env *env, const CovidBufs &fin, void *stream) {
-    aie_covid_step_final_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, fin);
+    if (env->obs_bf16) aie_covid_step_final_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, fin);
+    else aie_covid_step_final_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, fin);
     AIE_CUDA(cudaGetLastError(), "aie_covid_step_final_kernel launch");
     env->launches++;
     return AIE_OK;

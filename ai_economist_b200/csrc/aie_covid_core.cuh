@@ -108,39 +108,55 @@ CV_DEV int8_t cv_ring_at(const int8_t *ring, int head, int k, int L1, int S, int
     return ring[(size_t)a * cv_ring_row(L1) + p];
 }
 
-// Observations + masks of the current state (used after a step and after a reset).
+// Observations + masks of the current state (used after a step and after a reset).  OT: the element type of the seven
+// observation / mask tensors (float, or bf16_t under AIE_OBS_BF16): every value is computed as for float32 output and
+// rounded float32 -> bfloat16 on the way out (put_out), so a float64 intermediate is rounded to float32 first.
+template <typename OT = float>
 CV_DEV void covid_observe(const CovidCfg &c, const float *st, const int32_t *ints, const int32_t *hdr, const int8_t *ring,
                           int head, int e, const CovidBufs &b, int tid, int nthr) {
+    // Each value is computed before its destination address, the order of the float32 assignments this replaced.
     const int S = c.S, L1 = c.L + 1, t = hdr[CVH_T];
     for (int a = tid; a < S; a += nthr) {
         const double pop = (double)c.pop[a];
-        for (int k = 0; k < 6; k++)  // f64: float32 state / int32 population
-            b.o_state[((size_t)e * 6 + k) * S + a] = (float)((double)st[k * S + a] / pop);
-        b.o_post[(size_t)e * S + a] = st[CVS_POST * S + a] / c.max_prod[a];
+        for (int k = 0; k < 6; k++) {  // f64: float32 state / int32 population
+            const float v = (float)((double)st[k * S + a] / pop);
+            put_out((OT *)b.o_state + ((size_t)e * 6 + k) * S + a, v);
+        }
+        const float post = st[CVS_POST * S + a] / c.max_prod[a];
+        put_out((OT *)b.o_post + (size_t)e * S + a, post);
         const float lag = (float)cv_ring_at(ring, head, c.L - c.beta_delay + 1, L1, S, a);
-        b.o_lag[(size_t)e * S + a] = lag / (float)c.levels;
-        b.o_pol[(size_t)e * S + a] = st[CVS_STRG * S + a] / (float)c.levels;
+        const float lag_v = lag / (float)c.levels;
+        put_out((OT *)b.o_lag + (size_t)e * S + a, lag_v);
+        const float pol = st[CVS_STRG * S + a] / (float)c.levels;
+        put_out((OT *)b.o_pol + (size_t)e * S + a, pol);
         const float open = (t >= ints[a]) ? 1.0f : 0.0f;  // cooldown_until
-        float *m = b.mask_a + (size_t)e * (1 + c.levels) * S;
-        m[a] = 1.0f;
-        for (int l = 1; l <= c.levels; l++) m[(size_t)l * S + a] = open;
+        OT *m = (OT *)b.mask_a + (size_t)e * (1 + c.levels) * S;
+        put_out(m + a, 1.0f);
+        for (int l = 1; l <= c.levels; l++) put_out(m + (size_t)l * S + a, open);
     }
-    for (int j = tid; j <= c.sub_levels; j += nthr)
-        b.mask_p[(size_t)e * (1 + c.sub_levels) + j] = (j == 0 || (t % c.sub_interval) == 0) ? 1.0f : 0.0f;
+    for (int j = tid; j <= c.sub_levels; j += nthr) {
+        const float v = (j == 0 || (t % c.sub_interval) == 0) ? 1.0f : 0.0f;
+        put_out((OT *)b.mask_p + (size_t)e * (1 + c.sub_levels) + j, v);
+    }
     if (tid == 0) {
-        float *sc = b.o_scal + (size_t)e * 4;
-        sc[0] = (float)((double)t / c.time_scale);
-        sc[1] = (float)((double)(c.sub_interval - t % c.sub_interval) / (double)c.sub_interval);
-        sc[2] = (float)((double)hdr[CVH_SUBSIDY_LEVEL] / (double)c.sub_levels);
+        OT *sc = (OT *)b.o_scal + (size_t)e * 4;
+        const float s0 = (float)((double)t / c.time_scale);
+        put_out(sc + 0, s0);
+        const float s1 = (float)((double)(c.sub_interval - t % c.sub_interval) / (double)c.sub_interval);
+        put_out(sc + 1, s1);
+        const float s2 = (float)((double)hdr[CVH_SUBSIDY_LEVEL] / (double)c.sub_levels);
+        put_out(sc + 2, s2);
         const int nxt = t + 1;
         double tv;
         if (nxt <= c.t_first_delivery) tv = fmin(1.0, (double)(c.t_first_delivery - nxt) / (double)c.vac_interval);
         else tv = (double)(c.vac_interval - nxt % c.vac_interval);
-        sc[3] = (float)(tv / (double)c.vac_interval);
+        const float s3 = (float)(tv / (double)c.vac_interval);
+        put_out(sc + 3, s3);
     }
 }
 
 // env.reset(): covid19_env.py:1175-1290 (deterministic: initial series from the real-world data at start_date)
+template <typename OT = float>
 CV_DEV void covid_reset_env(const CovidCfg &c, int e, const CovidBufs &b, int tid, int nthr, bool keep_outputs) {
     const int S = c.S, L1 = c.L + 1;
     float *st = b.state + (size_t)e * CVS_FIELDS * S;
@@ -181,7 +197,7 @@ CV_DEV void covid_reset_env(const CovidCfg &c, int e, const CovidBufs &b, int ti
         if (!keep_outputs) { b.rew_p[e] = 0.0; b.done[e] = 0; }
     }
     cv_bsync();
-    covid_observe(c, st, ints, hdr, ring, 0, e, b, tid, nthr);
+    covid_observe<OT>(c, st, ints, hdr, ring, 0, e, b, tid, nthr);
 }
 
 // red: scratch float [3][S] (shared memory on the device)
@@ -203,8 +219,8 @@ CV_DEV double cv_accumulate_changes(const CovidCfg &c, const uint32_t *lst, int 
 constexpr int CV_CHG_CAP = 32;
 // FINAL: on the step that ends an episode under the auto-reset, first write the observations / masks of the state the
 // episode ended in into row e of fin's seven observation / mask tensors (fin: b with those pointers replaced), then
-// reset.  Unused without FINAL.
-template <bool FINAL>
+// reset.  Unused without FINAL.  OT: the element type of the observation / mask tensors (covid_observe).
+template <bool FINAL, typename OT = float>
 CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const CovidBufs &fin, float *red, uint32_t *chg,
                            int tid, int nthr) {
     const int S = c.S, L = c.L, L1 = c.L + 1, F = c.F;
@@ -393,13 +409,13 @@ CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const C
         // the ordinary steps of this kernel 7.7 % slower on an H100 (the code ptxas makes of the whole body); this form
         // leaves them unchanged (DESIGN §6).
         const bool end = c.auto_reset && t >= c.T;
-        covid_observe(c, st, ints, hdr, ring, new_head, e, end ? fin : b, tid, nthr);
+        covid_observe<OT>(c, st, ints, hdr, ring, new_head, e, end ? fin : b, tid, nthr);
         if (end) {
             cv_bsync();   // once per episode: the reset below overwrites what the final pass reads
-            covid_reset_env(c, e, b, tid, nthr, true);
+            covid_reset_env<OT>(c, e, b, tid, nthr, true);
         }
-    } else if (c.auto_reset && t >= c.T) covid_reset_env(c, e, b, tid, nthr, true);
-    else covid_observe(c, st, ints, hdr, ring, new_head, e, b, tid, nthr);
+    } else if (c.auto_reset && t >= c.T) covid_reset_env<OT>(c, e, b, tid, nthr, true);
+    else covid_observe<OT>(c, st, ints, hdr, ring, new_head, e, b, tid, nthr);
 }
 // The step without final observations (aie_covid_step).
 CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, float *red, uint32_t *chg, int tid, int nthr) {
@@ -413,16 +429,18 @@ CV_DEV uint64_t cv_mix64(uint64_t x) {
     x = (x ^ (x >> 27)) * 0x94d049bb133111ebull;
     return x ^ (x >> 31);
 }
+// MT: the element type of the masks (float, or bf16_t under AIE_OBS_BF16).
+template <typename MT = float>
 CV_DEV void covid_sample_env(const CovidCfg &c, int e, const CovidBufs &b, uint64_t key, int tid, int nthr) {
     const int S = c.S;
     int32_t *act_a = const_cast<int32_t *>(b.act_a) + (size_t)e * S;
     for (int a = tid; a < S; a += nthr) {
-        const bool open = b.mask_a[((size_t)e * (1 + c.levels) + 1) * S + a] != 0.0f;
+        const bool open = mask_open(((const MT *)b.mask_a)[((size_t)e * (1 + c.levels) + 1) * S + a]);
         const uint32_t r = (uint32_t)(cv_mix64(key + 0x100 * (uint64_t)a) >> 32);
         act_a[a] = open ? (int32_t)(r % (uint32_t)(1 + c.levels)) : 0;
     }
     if (tid == 0) {
-        const bool open = b.mask_p[(size_t)e * (1 + c.sub_levels) + 1] != 0.0f;
+        const bool open = mask_open(((const MT *)b.mask_p)[(size_t)e * (1 + c.sub_levels) + 1]);
         const uint32_t r = (uint32_t)(cv_mix64(key ^ 0xabcdefull) >> 32);
         const_cast<int32_t *>(b.act_p)[e] = open ? (int32_t)(r % (uint32_t)(1 + c.sub_levels)) : 0;
     }
@@ -431,18 +449,19 @@ CV_DEV void covid_sample_env(const CovidCfg &c, int e, const CovidBufs &b, uint6
 // Policy sampler (aie_covid_sample_policy, policy_segment_warp in aie_core.cuh): unit u < S draws state u's stringency
 // level from its logits [E][S][1 + levels] under the mask column mask_a[e][.][u]; unit S draws the planner's subsidy
 // level from [E][1 + sub_levels].  Keys as covid_sample_env: key + 0x100 * u for a state, key ^ 0xabcdef for the planner.
-template <typename LT>
+// LT: the logits' element type; MT: the masks' (float, or bf16_t under AIE_OBS_BF16).
+template <typename LT, typename MT = float>
 CV_DEV void covid_policy_unit(const CovidCfg &c, int e, const CovidBufs &b, const PolicyBufs &p, uint64_t key, int u, int lane) {
     float lp;
     if (u < c.S) {
         const int n = 1 + c.levels;
         const size_t i = (size_t)e * c.S + u;
-        const int v = policy_segment_warp(b.mask_a + (size_t)e * n * c.S + u, c.S, (const LT *)p.a_logit + i * n, n,
+        const int v = policy_segment_warp((const MT *)b.mask_a + (size_t)e * n * c.S + u, c.S, (const LT *)p.a_logit + i * n, n,
                                           key + 0x100 * (uint64_t)u, p.greedy, lane, &lp);
         if (lane == 0) { const_cast<int32_t *>(b.act_a)[i] = v; if (p.lp_a) p.lp_a[i] = lp; }
     } else {
         const int n = 1 + c.sub_levels;
-        const int v = policy_segment_warp(b.mask_p + (size_t)e * n, 1, (const LT *)p.p_logit + (size_t)e * n, n,
+        const int v = policy_segment_warp((const MT *)b.mask_p + (size_t)e * n, 1, (const LT *)p.p_logit + (size_t)e * n, n,
                                           key ^ 0xabcdefull, p.greedy, lane, &lp);
         if (lane == 0) { const_cast<int32_t *>(b.act_p)[e] = v; if (p.lp_p) p.lp_p[e] = lp; }
     }

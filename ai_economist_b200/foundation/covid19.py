@@ -213,7 +213,9 @@ class CovidBatchedEnv:
 
     Observations come collated exactly like the reference's mandatory `collate_agent_step_and_reset_data=True`
     layout: obs["a"][key] has the agent (US state) axis last, obs["p"][key] is the planner's; every tensor has
-    a leading env axis.  Values are float32 (the reference's own CUDA path also uses float32 placeholders).
+    a leading env axis.  Values are float32 (the reference's own CUDA path also uses float32 placeholders), or with
+    obs_dtype=torch.bfloat16 bfloat16: every observation and mask element is the round-to-nearest-even bfloat16 of the
+    float32 value, written by the step kernel itself (rewards, done and actions are unchanged).
     """
 
     def __init__(self, components=None, n_agents=51, world_size=(1, 1), episode_length=540,
@@ -223,8 +225,7 @@ class CovidBatchedEnv:
                  stepper_factory=None, seed=None, seeds=None, dense_log_frequency=None, world_dense_log_frequency=50,
                  obs_dtype=None, final_obs=False, **scenario_kwargs):
         from .._abi import obs_dtype_name
-        if obs_dtype_name(obs_dtype) != "float32":
-            raise NotImplementedError("the COVID-19 scenario writes float32 observations only")
+        self._obs_dtype = obs_dtype_name(obs_dtype)
         if final_obs and not auto_reset:
             raise ValueError("final_obs=True needs auto_reset=True: without the auto-reset, env.obs after the step that "
                              "ends an episode already is its final observation")
@@ -261,14 +262,22 @@ class CovidBatchedEnv:
         if stepper_factory is None:
             from ..covid_stepper import CudaCovidStepper
             self._stepper = CudaCovidStepper(self.params, self.n_envs, device=device, auto_reset=auto_reset,
-                                             final_obs=bool(final_obs))
-        elif final_obs:
-            self._stepper = stepper_factory(self.params, self.n_envs, auto_reset, final_obs=True)
-            if not getattr(self._stepper, "final_obs", False):
+                                             final_obs=bool(final_obs), obs_dtype=self._obs_dtype)
+        else:
+            # a factory gets final_obs / obs_dtype only when they differ from the defaults, so a three-argument
+            # factory keeps working for a default env
+            kw = {}
+            if final_obs:
+                kw["final_obs"] = True
+            if self._obs_dtype != "float32":
+                kw["obs_dtype"] = self._obs_dtype
+            self._stepper = stepper_factory(self.params, self.n_envs, auto_reset, **kw)
+            if final_obs and not getattr(self._stepper, "final_obs", False):
                 raise NotImplementedError("final_obs=True: the stepper made by stepper_factory does not write final "
                                           "observations (it needs final_<name> buffers and a final-observation step)")
-        else:
-            self._stepper = stepper_factory(self.params, self.n_envs, auto_reset)
+            if getattr(self._stepper, "obs_dtype", "float32") != self._obs_dtype:
+                raise NotImplementedError("obs_dtype=%s: the stepper made by stepper_factory writes %s observations"
+                                          % (self._obs_dtype, getattr(self._stepper, "obs_dtype", "float32")))
         self._final_obs = bool(final_obs)
         self._loaded = False
         self._build_views()
@@ -353,7 +362,9 @@ class CovidBatchedEnv:
     def _build_rate_observation(self):
         """VaccinationCampaign(observe_rate=True) (covid19_components.py:629-661): the vaccination rate of the NEXT timestep, 0
         until deliveries have begun.  It depends on the timestep alone, so it is a table lookup by the replica's timestep after
-        every step / reset (the reference's own CUDA path does not emit it; no kernel involved)."""
+        every step / reset (the reference's own CUDA path does not emit it; no kernel involved).  The table and the rate
+        tensors have the observations' element type: under bfloat16 each entry is the round-to-nearest-even of the
+        float32 rate (raw bits on numpy backends, as the stepper's observation buffers)."""
         vac = self._components[2]
         self._rate_tab = None
         if not vac.observe_rate:
@@ -364,11 +375,14 @@ class CovidBatchedEnv:
         sc = self._stepper.buf["obs_scalars"]
         E, S = self.n_envs, self.n_agents
         if isinstance(sc, np.ndarray):
-            self._rate_tab, self._rate_a, self._rate_p = tab, np.zeros((E, S), np.float32), np.zeros(E, np.float32)
+            if sc.dtype == np.uint16:   # raw bfloat16 bits, rounded to nearest even (the rates are finite)
+                u = tab.view(np.uint32)
+                tab = ((u + np.uint32(0x7FFF) + ((u >> 16) & np.uint32(1))) >> 16).astype(np.uint16)
+            self._rate_tab, self._rate_a, self._rate_p = tab, np.zeros((E, S), tab.dtype), np.zeros(E, tab.dtype)
         else:
             import torch
-            self._rate_tab = torch.as_tensor(tab, device=sc.device)
-            self._rate_a, self._rate_p = torch.zeros((E, S), dtype=torch.float32, device=sc.device), torch.zeros(E, dtype=torch.float32, device=sc.device)
+            self._rate_tab = torch.as_tensor(tab, device=sc.device).to(sc.dtype)
+            self._rate_a, self._rate_p = torch.zeros((E, S), dtype=sc.dtype, device=sc.device), torch.zeros(E, dtype=sc.dtype, device=sc.device)
         self.obs["a"]["VaccinationCampaign-next_vaccination_rate"] = self._rate_a
         self.obs["p"]["VaccinationCampaign-next_vaccination_rate"] = self._rate_p
         if self.final_obs is not None:
@@ -379,20 +393,24 @@ class CovidBatchedEnv:
             self.final_obs["a"]["VaccinationCampaign-next_vaccination_rate"] = self._final_rate_a
             self.final_obs["p"]["VaccinationCampaign-next_vaccination_rate"] = self._final_rate_p
 
-    def _rate_of(self, sc):
-        """The table's rate at the timesteps of obs_scalars sc: [:, 0] = timestep / time_scale (episode_length under
-        observation scaling)."""
+    def _timesteps(self):
+        """Each replica's timestep: from the float32 time scalar t / time_scale, which holds it exactly, or under bfloat16
+        observations from hdr[:, 0] (a bfloat16 t / 540 spans one to two timesteps)."""
+        b = self._stepper.buf
+        sc = b["obs_scalars"]
         scale = float(self.params["time_scale"])
         if isinstance(sc, np.ndarray):
-            return self._rate_tab[np.rint(sc[:, 0].astype(np.float64) * scale).astype(np.int64)]
+            return b["hdr"][:, 0] if sc.dtype == np.uint16 else np.rint(sc[:, 0].astype(np.float64) * scale).astype(np.int64)
         import torch
-        return self._rate_tab[torch.round(sc[:, 0].double() * scale).long()]
+        return b["hdr"][:, 0].long() if sc.dtype == torch.bfloat16 else torch.round(sc[:, 0].double() * scale).long()
 
     def _refresh_rate_observation(self, stepped=False):
+        """The table's rates at each replica's timestep.  The final rows are those of episodes that ended on their time
+        limit, so their rate is the table's last entry (t = episode_length)."""
         if self._rate_tab is None:
             return
         b = self._stepper.buf
-        rate = self._rate_of(b["obs_scalars"])
+        rate = self._rate_tab[self._timesteps()]
         if isinstance(rate, np.ndarray):
             self._rate_p[...] = rate
             self._rate_a[...] = self._rate_p[:, None]
@@ -400,16 +418,16 @@ class CovidBatchedEnv:
             self._rate_p.copy_(rate)
             self._rate_a.copy_(self._rate_p[:, None].expand_as(self._rate_a))
         if stepped and self.final_obs is not None:
-            # only the rows of the episodes this step ended: their own time scalar is t = T (the table's last entry)
+            # only the rows of the episodes this step ended
             done = b["done"] != 0
-            rate = self._rate_of(b["final_obs_scalars"])
-            if isinstance(rate, np.ndarray):
-                self._final_rate_p[...] = np.where(done, rate, self._final_rate_p)
-                self._final_rate_a[...] = np.where(done[:, None], rate[:, None], self._final_rate_a)
+            last = self._rate_tab[self._episode_length]
+            if isinstance(done, np.ndarray):
+                self._final_rate_p[...] = np.where(done, last, self._final_rate_p)
+                self._final_rate_a[...] = np.where(done[:, None], last, self._final_rate_a)
             else:
                 import torch
-                self._final_rate_p.copy_(torch.where(done, rate, self._final_rate_p))
-                self._final_rate_a.copy_(torch.where(done[:, None], rate[:, None], self._final_rate_a))
+                self._final_rate_p.copy_(torch.where(done, last, self._final_rate_p))
+                self._final_rate_a.copy_(torch.where(done[:, None], last, self._final_rate_a))
 
     def reset(self):
         self._stepper.reset()

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define AIE_ABI_VERSION 5
+#define AIE_ABI_VERSION 6
 
 #define AIE_MAX_COMPONENTS 8
 #define AIE_MAX_BRACKETS 16
@@ -599,13 +599,22 @@ typedef struct aie_covid_config {
     const double *max_daily_subsidy_per_state;
     const int8_t *rw_policy;        /* [rw_policy_days, S] real-world stringency (initial history, lag before t = beta_delay) */
     const float *init_state;        /* [6, S] Susceptible, Infected, Recovered, Deaths, Vaccinated, Unemployed at t = 0 */
+    /* ABI 6.  Element type of the seven observation / mask tensors, obs_agent_state .. mask_planner, of aie_covid_buffers
+     * and of aie_covid_obs_buffers: AIE_OBS_F32 (default), or AIE_OBS_BF16 - every element is the round-to-nearest-even
+     * bfloat16 of the float32 the default writes (a value computed in float64 is rounded to float32 first, then to
+     * bfloat16), converted by the kernels that write it (same launches, half the bytes).  State, ints, hdr, ring,
+     * changes, rewards, done and actions are unchanged; the masks are 0 / 1, so both samplers draw the same actions.
+     * Any other value: AIE_EINVAL at aie_covid_create. */
+    int32_t obs_dtype;
 } aie_covid_config;
 
 /* Device buffers (contiguous, env-major).  state: float32 [E, 9, S] = S, I, R, D, V, U, stringency, subsidy,
  * postsubsidy productivity at the current timestep; ints: int32 [E, 2, S] = cooldown_until, vaccines_available;
  * hdr: int32 [E, 4] = t, subsidy_level, ring_head, episodes; ring: int8 [E, S, ROW] stringency history, time-minor
  * (ROW = filter_len + 1 rounded up to a multiple of 16 bytes; logical entry k sits at column (ring_head + k) mod (L+1)).
- * Observations are the reference's collated "a"/"p" fields (covid19_env.py:919-993 + components), float32. */
+ * Observations are the reference's collated "a"/"p" fields (covid19_env.py:919-993 + components), float32; with
+ * aie_covid_config::obs_dtype == AIE_OBS_BF16 the seven float* observation / mask pointers point to bfloat16 storage
+ * (2 bytes per element, same shapes). */
 typedef struct aie_covid_buffers {
     float *state; int32_t *ints; int32_t *hdr; int8_t *ring;
     const int32_t *actions_agent;   /* [E, S] stringency action 0..num_stringency_levels (0 = NO-OP) */
@@ -636,7 +645,8 @@ int aie_covid_reset(aie_covid_env *env, void *stream);
 /* One env.step() for every replica: 3 component steps + scenario step + observations + rewards + done. */
 int aie_covid_step(aie_covid_env *env, void *stream);
 
-/* The seven observation / mask tensors of aie_covid_buffers, with the same shapes, float32. */
+/* The seven observation / mask tensors of aie_covid_buffers, with the same shapes and element type (float32, or
+ * bfloat16 storage under AIE_OBS_BF16). */
 typedef struct aie_covid_obs_buffers {
     float *obs_agent_state, *obs_postsubsidy, *obs_lagged_stringency, *obs_policy_indicators, *obs_scalars,
           *mask_agent, *mask_planner;
@@ -646,8 +656,9 @@ typedef struct aie_covid_obs_buffers {
  * done flag this step sets, row e of `final_out` receives what aie_covid_step writes for that env with auto_reset off
  * (the observations and masks of the state its episode ended in; the bound tensors already show the next episode's
  * first).  Rows of the other envs are left untouched.  What a trainer bootstraps a truncated episode's value from.
- * One launch, asynchronous on `stream`.  AIE_EINVAL for a NULL env or final_out, a NULL member or a member not 4-byte
- * aligned; AIE_ESTATE before buffers are bound and the env has been reset, or with auto_reset off. */
+ * One launch, asynchronous on `stream`.  AIE_EINVAL for a NULL env or final_out, a NULL member or a member not aligned
+ * to its element (4 bytes, 2 under AIE_OBS_BF16); AIE_ESTATE before buffers are bound and the env has been reset, or
+ * with auto_reset off. */
 int aie_covid_step_final(aie_covid_env *env, const aie_covid_obs_buffers *final_out, void *stream);
 /* Random policy on the device (uniform over the unmasked actions of the current masks); see aie_sample_random_actions. */
 int aie_covid_sample_random_actions(aie_covid_env *env, uint64_t seed, void *stream);
