@@ -122,6 +122,12 @@ class AieObsBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in OBS_NAMES]
 
 
+class AieRollout(C.Structure):
+    """aie_rollout: the device tensors of a rollout stored in place (aie_bind_rollout)."""
+    _fields_ = [("T", C.c_int32), ("obs", AieObsBuffers), ("actions_agent", C.c_void_p), ("actions_planner", C.c_void_p),
+                ("reward", C.c_void_p), ("done", C.c_void_p), ("final_obs", AieObsBuffers)]
+
+
 class AiePolicyLogits(C.Structure):
     _fields_ = [("agent", C.c_void_p), ("planner", C.c_void_p), ("logits_dtype", C.c_int32), ("greedy", C.c_int32),
                 ("log_prob_agent", C.c_void_p), ("log_prob_planner", C.c_void_p)]
@@ -182,6 +188,13 @@ class AieCovidObsBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in COVID_OBS_NAMES]
 
 
+class AieCovidRollout(C.Structure):
+    """aie_covid_rollout: the device tensors of a COVID-19 rollout stored in place (aie_covid_bind_rollout)."""
+    _fields_ = [("T", C.c_int32), ("obs", AieCovidObsBuffers), ("actions_agent", C.c_void_p),
+                ("actions_planner", C.c_void_p), ("reward_agent", C.c_void_p), ("reward_planner", C.c_void_p),
+                ("done", C.c_void_p), ("final_obs", AieCovidObsBuffers)]
+
+
 class AieError(RuntimeError):
     pass
 
@@ -225,6 +238,18 @@ def load_library(path=None):
     for fn in ["aie_compute_advantages", "aie_covid_compute_advantages"]:
         getattr(L, fn).argtypes = [P, C.POINTER(AieAdvantageArgs), C.c_int32, P]
         getattr(L, fn).restype = C.c_int
+    L.aie_compute_advantages_k.argtypes = [P, C.POINTER(AieAdvantageArgs), C.c_int32, C.c_int32, P]
+    L.aie_compute_advantages_k.restype = C.c_int
+    L.aie_bind_rollout.argtypes = [P, C.POINTER(AieRollout)]
+    L.aie_bind_rollout.restype = C.c_int
+    L.aie_rollout_restart.argtypes = [P, P]
+    L.aie_rollout_restart.restype = C.c_int
+    L.aie_covid_compute_advantages_k.argtypes = [P, C.POINTER(AieAdvantageArgs), C.c_int32, C.c_int32, P]
+    L.aie_covid_compute_advantages_k.restype = C.c_int
+    L.aie_covid_bind_rollout.argtypes = [P, C.POINTER(AieCovidRollout)]
+    L.aie_covid_bind_rollout.restype = C.c_int
+    L.aie_covid_rollout_restart.argtypes = [P, P]
+    L.aie_covid_rollout_restart.restype = C.c_int
     L.aie_step_host.argtypes = [P, P, P, C.POINTER(AieHostOut), P]
     L.aie_step_host_compact.argtypes = [P, P, P, C.POINTER(AieHostOut), C.c_int32, P]
     L.aie_step_host_compact.restype = C.c_int
@@ -264,11 +289,12 @@ def load_library(path=None):
 
 EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field", "aie_get_flat_layout", "aie_bind_buffers",
                     "aie_load_state", "aie_reset_envs", "aie_step", "aie_step_dynamics", "aie_observe", "aie_observe_final", "aie_sample_random_actions",
-                    "aie_set_fused_policy", "aie_sample_policy", "aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_compute_advantages", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
+                    "aie_set_fused_policy", "aie_sample_policy", "aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_compute_advantages", "aie_compute_advantages_k", "aie_bind_rollout", "aie_rollout_restart", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
                     "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
                     "aie_covid_step_final", "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
-                    "aie_covid_evaluate_policy_backward", "aie_covid_compute_advantages", "aie_covid_launch_count"]
+                    "aie_covid_evaluate_policy_backward", "aie_covid_compute_advantages", "aie_covid_launch_count",
+                    "aie_covid_bind_rollout", "aie_covid_rollout_restart", "aie_covid_compute_advantages_k"]
 
 
 def obs_dtype_name(obs_dtype):

@@ -237,6 +237,10 @@ class ReferenceApiEnv:
     def __getattr__(self, name):           # get_agent, n_agents, episode_length, world, metrics, dense logs, seed ...
         return getattr(self._env, name)
 
+    def bind_rollout(self, T, final_obs=False):
+        raise NotImplementedError("the reference API steps one replica through host copies; bind rollouts on the "
+                                  "batched env (reference_api=False)")
+
     @property
     def _completions(self):                # int, like the reference's (tutorials/rllib/env_wrapper.py:176 reads it)
         return int(self._env.completions()[self._e])

@@ -1,10 +1,11 @@
 """Python driver of the COVID-19 scenario kernels (plumbing: buffers + ABI calls)."""
 import ctypes as C
+import numbers
 
 import numpy as np
 
 from . import _abi
-from .stepper import PolicySampler, bf16_bits_to_float32, buf_kind_torch, float_kind_torch, is_i32_torch
+from .stepper import PolicySampler, Rollout, bf16_bits_to_float32, buf_kind_torch, float_kind_torch, is_i32_torch
 
 F32, I32 = np.float32, np.int32
 
@@ -112,6 +113,9 @@ class CovidStepperBase(PolicySampler):
         if self.change_list:
             shapes["changes"] = ("i32", (E, 33, S))
         self.buf = {k: self._alloc(shape, dt) for k, (dt, shape) in shapes.items()}
+        self._shapes = shapes
+        self.rollout = None   # the bound Rollout (bind_rollout), and its slot cursor
+        self.rollout_slot = 0
         bufs = _abi.AieCovidBuffers()
         for name in _abi._COVID_BUF_NAMES:
             setattr(bufs, name, self._ptr(self.buf[name]))
@@ -145,10 +149,48 @@ class CovidStepperBase(PolicySampler):
         self._check(self.lib.aie_covid_reset(self._h, self._stream()))
 
     def step(self):
-        if self.final_obs:
+        if self.rollout is not None:   # slot s -> s + 1; the final observations go to the rollout's final slots
+            self._check(self.lib.aie_covid_step(self._h, self._stream()))
+            self.rollout_slot += 1
+        elif self.final_obs:
             self._check(self.lib.aie_covid_step_final(self._h, C.byref(self._final_bufs), self._stream()))
         else:
             self._check(self.lib.aie_covid_step(self._h, self._stream()))
+
+    # -- rollouts stored in place (aie_covid_bind_rollout) -----------------------------------------------------------
+    def bind_rollout(self, T, final_obs=False):
+        """Allocate and bind a rollout of T steps (a Rollout), with final slots [K, E, ...] when final_obs."""
+        if isinstance(T, bool) or not isinstance(T, numbers.Integral) or T < 1:
+            raise ValueError("T must be a positive int")
+        if self.rollout is not None:
+            raise ValueError("a rollout is already bound: unbind_rollout() first")
+        T = int(T)
+        K = -(-T // int(self.p["episode_length"]))
+        sh, names = self._shapes, list(_abi.COVID_OBS_NAMES)
+        buf = {k: self._alloc((T + 1,) + sh[k][1], sh[k][0]) for k in names}
+        for k in ("actions_agent", "actions_planner", "reward_agent", "reward_planner", "done"):
+            buf[k] = self._alloc((T,) + sh[k][1], sh[k][0])
+        r = _abi.AieCovidRollout()
+        r.T = T
+        for k in names:
+            setattr(r.obs, k, self._ptr(buf[k]))
+        if final_obs:
+            for k in names:
+                buf["final_" + k] = self._alloc((K,) + sh[k][1], sh[k][0])
+                setattr(r.final_obs, k, self._ptr(buf["final_" + k]))
+        for k in ("actions_agent", "actions_planner", "reward_agent", "reward_planner", "done"):
+            setattr(r, k, self._ptr(buf[k]))
+        self._check(self.lib.aie_covid_bind_rollout(self._h, C.byref(r)))
+        self.rollout, self.rollout_slot = Rollout(T, K, buf, names, bool(final_obs)), 0
+        return self.rollout
+
+    def restart_rollout(self):
+        self._check(self.lib.aie_covid_rollout_restart(self._h, self._stream()))
+        self.rollout_slot = 0
+
+    def unbind_rollout(self):
+        self._check(self.lib.aie_covid_bind_rollout(self._h, None))
+        self.rollout, self.rollout_slot = None, 0
 
     def sample_random_actions(self, seed=0):
         self._check(self.lib.aie_covid_sample_random_actions(self._h, C.c_uint64(int(seed)), self._stream()))
@@ -170,6 +212,10 @@ class CovidStepperBase(PolicySampler):
     @property
     def _adv_fn(self):
         return self.lib.aie_covid_compute_advantages
+
+    @property
+    def _adv_k_fn(self):
+        return self.lib.aie_covid_compute_advantages_k
 
     def _mask_rows(self):   # evaluate_policy: the agent mask is [*B, 1 + levels, S], transposed against the logits
         S, L = self.p["n_states"], self.p["num_stringency_levels"]

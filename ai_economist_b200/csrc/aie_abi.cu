@@ -30,6 +30,10 @@
 //                          with their float32 twins' launch shapes.
 //   aie_compute_advantages_kernel  one thread per column of a stored rollout (agent and planner columns, group-uniform
 //                          CTAs): advantages and value targets (aie_compute_advantages, aie_covid_compute_advantages).
+//   aie_observe_final_slot_kernel  aie_observe_final_kernel's shape and body, writing into a bound rollout's final slots:
+//                          row (k, e), k = the env's earlier done flags in the rollout (aie_bind_rollout).
+//   aie_compute_advantages_k_kernel  aie_compute_advantages_kernel with final values [K][n] indexed by episode-end
+//                          ordinal (aie_compute_advantages_k).
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
 // aie_config::obs_dtype == AIE_OBS_BF16); the launchers pick one from the config, with the same launch shape.
 #include <cuda_runtime.h>
@@ -120,6 +124,8 @@ int launch_policy_eval(aie_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_b
 int covid_launch_policy_eval(aie_covid_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows,
                              void *stream);
 int launch_advantages(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, void *stream);
+int launch_advantages_k(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, int K, void *stream);
+int launch_observe_final_slots(aie_env *, const DevBufs &fb, const int32_t *done0, int s, int K, void *stream);
 }  // namespace be
 }  // namespace aie
 
@@ -491,11 +497,23 @@ __global__ void __launch_bounds__(256) aie_observe_bf16_kernel(const __grid_cons
 }
 // FINAL (aie_observe_final_kernel): b's record source is episode_final and its outputs are the caller's final tensors;
 // a CTA whose env's done flag is zero leaves before it loads anything or writes any output.
-template <bool EXT, typename OT, bool FINAL = false>
-__device__ __forceinline__ void observe_mw_kernel_body(const DevCfg &c, const DevBufs &b, int lo, int n) {
+// SLOT (aie_observe_final_slot_kernel): FINAL into a rollout's final slots, b's outputs at slot 0 of them and b.done at
+// slot s of the rollout's dones (done0 at slot 0): the env's row is (k, env), k = its done flags in slots 0 .. s - 1; a
+// CTA with k >= nk leaves.
+template <bool EXT, typename OT, bool FINAL = false, bool SLOT = false>
+__device__ __forceinline__ void observe_mw_kernel_body(const DevCfg &c, const DevBufs &b, int lo, int n,
+                                                       const int32_t *done0 = nullptr, int s = 0, int nk = 0) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int env = lo + blockIdx.x;
     if constexpr (FINAL) { if (b.done[env] == 0) return; }   // one env per CTA: the whole CTA leaves
+    int k = 0;
+    if constexpr (SLOT) {
+        for (int t0 = 0; t0 < s; t0 += blockDim.x) {
+            const int t = t0 + threadIdx.x;
+            k += __syncthreads_count(t < s && done0[(size_t)t * c.n_envs + env] != 0);
+        }
+        if (k >= nk) return;   // uniform across the CTA
+    }
     const uint16_t *tab = stage_tables(smem, 1, c, b);
     uint64_t *bar = (uint64_t *)smem;
     uint8_t *rec = warp_region(smem, 1, 0, c);
@@ -503,7 +521,9 @@ __device__ __forceinline__ void observe_mw_kernel_body(const DevCfg &c, const De
     if (threadIdx.x == 0) load_obs_prefix(c, rec, grec, bar);
     __syncthreads();
     mbar_wait(bar, 0);
-    observe_env<EXT, CS_ALL, OT>(c, rec, grec, rec, c.ob, obs_out_for(c, b, env), tab, DevExec<128, false>{(int)threadIdx.x});
+    ObsOut o = obs_out_for(c, b, env);
+    if constexpr (SLOT) o.env += (size_t)k * c.n_envs;
+    observe_env<EXT, CS_ALL, OT>(c, rec, grec, rec, c.ob, o, tab, DevExec<128, false>{(int)threadIdx.x});
 }
 template <bool EXT>
 __global__ void __launch_bounds__(128, 4) aie_observe_mw_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
@@ -524,6 +544,12 @@ __global__ void __launch_bounds__(128, 4) aie_observe_final_kernel(const __grid_
 template <bool EXT>
 __global__ void __launch_bounds__(128, 4) aie_observe_final_bf16_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b, int lo, int n) {
     observe_mw_kernel_body<EXT, bf16_t, true>(c, b, lo, n);
+}
+// The final pass of a step into a bound rollout's final slots (aie_bind_rollout): aie_observe_final_kernel's shape.
+template <bool EXT, typename OT>
+__global__ void __launch_bounds__(128, 4) aie_observe_final_slot_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ DevBufs b,
+                                                                        const int32_t *done0, int s, int nk) {
+    observe_mw_kernel_body<EXT, OT, true, true>(c, b, 0, c.n_envs, done0, s, nk);
 }
 
 // Episode metrics (aie_metrics.cuh): one warp per env, eight per CTA, reads the env's record (current or end-of-episode
@@ -702,6 +728,8 @@ int init(aie_env *env) {
     AIE_OPT_IN(aie_observe_mw_bf16_kernel<false>); AIE_OPT_IN(aie_observe_mw_bf16_kernel<true>);
     AIE_OPT_IN(aie_observe_final_kernel<false>); AIE_OPT_IN(aie_observe_final_kernel<true>);
     AIE_OPT_IN(aie_observe_final_bf16_kernel<false>); AIE_OPT_IN(aie_observe_final_bf16_kernel<true>);
+    AIE_OPT_IN((aie_observe_final_slot_kernel<false, float>)); AIE_OPT_IN((aie_observe_final_slot_kernel<true, float>));
+    AIE_OPT_IN((aie_observe_final_slot_kernel<false, bf16_t>)); AIE_OPT_IN((aie_observe_final_slot_kernel<true, bf16_t>));
 #undef AIE_OPT_IN
     {
         AIE_CUDA(cudaMalloc((void **)&env->be.tab_dev, sizeof(Tables)), "cudaMalloc tables");
@@ -918,6 +946,20 @@ int launch_observe_final(aie_env *env, const DevBufs &fb, void *stream) {
     } else if (env->cfg.ext) aie_observe_final_kernel<true><<<n, 128, sm, st>>>(env->cfg, fb, 0, n);
     else aie_observe_final_kernel<false><<<n, 128, sm, st>>>(env->cfg, fb, 0, n);
     AIE_CUDA(cudaGetLastError(), "aie_observe_final_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+// aie_observe_final_slot_kernel: launch_observe_final's shape
+int launch_observe_final_slots(aie_env *env, const DevBufs &fb, const int32_t *done0, int s, int K, void *stream) {
+    const int n = env->n_envs;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t sm = env->be.env_cta_smem;
+    if (env->cfg.obs_bf16) {
+        if (env->cfg.ext) aie_observe_final_slot_kernel<true, bf16_t><<<n, 128, sm, st>>>(env->cfg, fb, done0, s, K);
+        else aie_observe_final_slot_kernel<false, bf16_t><<<n, 128, sm, st>>>(env->cfg, fb, done0, s, K);
+    } else if (env->cfg.ext) aie_observe_final_slot_kernel<true, float><<<n, 128, sm, st>>>(env->cfg, fb, done0, s, K);
+    else aie_observe_final_slot_kernel<false, float><<<n, 128, sm, st>>>(env->cfg, fb, done0, s, K);
+    AIE_CUDA(cudaGetLastError(), "aie_observe_final_slot_kernel launch");
     env->launches++;
     return AIE_OK;
 }
@@ -1176,7 +1218,32 @@ __global__ void __launch_bounds__(256) aie_compute_advantages_kernel(const __gri
         if (col < b.n[1]) gae_column<RP>(b, 1, E, col, T);
     }
 }
+// aie_compute_advantages_k: the same launch shape, final values [nk][n] by episode-end ordinal.
+template <typename RA, typename RP>
+__global__ void __launch_bounds__(256) aie_compute_advantages_k_kernel(const __grid_constant__ AdvantageBufs b, long long E,
+                                                                       int T, unsigned cta_a, int nk) {
+    if (blockIdx.x < cta_a) {
+        const long long col = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+        if (col < b.n[0]) gae_column<RA, true>(b, 0, E, col, T, nk);
+    } else {
+        const long long col = (long long)(blockIdx.x - cta_a) * blockDim.x + threadIdx.x;
+        if (col < b.n[1]) gae_column<RP, true>(b, 1, E, col, T, nk);
+    }
+}
 namespace be {
+int launch_advantages_k(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, int K, void *stream) {
+    const long long cta_a = (b.n[0] + 255) / 256, cta_p = (b.n[1] + 255) / 256;
+    if (cta_a + cta_p > 0x7fffffffLL) return fail(AIE_EINVAL, "aie_compute_advantages_k: too many columns for one launch");
+    const unsigned grid = (unsigned)(cta_a + cta_p), ca = (unsigned)cta_a;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (ra64) {
+        if (rp64) aie_compute_advantages_k_kernel<double, double><<<grid, 256, 0, st>>>(b, E, T, ca, K);
+        else aie_compute_advantages_k_kernel<double, float><<<grid, 256, 0, st>>>(b, E, T, ca, K);
+    } else if (rp64) aie_compute_advantages_k_kernel<float, double><<<grid, 256, 0, st>>>(b, E, T, ca, K);
+    else aie_compute_advantages_k_kernel<float, float><<<grid, 256, 0, st>>>(b, E, T, ca, K);
+    AIE_CUDA(cudaGetLastError(), "aie_compute_advantages_k_kernel launch");
+    return AIE_OK;
+}
 int launch_advantages(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, void *stream) {
     const long long cta_a = (b.n[0] + 255) / 256, cta_p = (b.n[1] + 255) / 256;
     if (cta_a + cta_p > 0x7fffffffLL) return fail(AIE_EINVAL, "aie_compute_advantages: too many columns for one launch");

@@ -2051,12 +2051,21 @@ AIE_DEV void gae_load_vals(RT *r, float *v, float *f, const int32_t *d, const RT
 // One column of group g over T steps (the recursion of aie_compute_advantages, include/aie_b200.h).  The carry is
 // only A and the value of the next row; the dones run one chunk ahead of the other loads so that the final values of
 // a chunk can be fetched as soon as its rewards and values are.
-template <typename RT>
-AIE_DEV void gae_column(const AdvantageBufs &b, int g, long long E, long long col, int T) {
+// KF (aie_compute_advantages_k): the final values are [nk][n], row = the done's episode-end ordinal in the column: the
+// column's done count is taken first, and a done step reads its row when the recursion reaches it (an ordinal >= nk
+// reads NaN).
+template <typename RT, bool KF = false>
+AIE_DEV void gae_column(const AdvantageBufs &b, int g, long long E, long long col, int T, int nk = 0) {
     constexpr int K = AIE_GAE_K;
     const long long n = b.n[g], e = col / b.per_env[g];
     const RT *R = (const RT *)b.r[g];
-    const float *V = b.v[g], *F = b.fv[g];
+    const float *V = b.v[g], *F = KF ? nullptr : b.fv[g];
+    const float *FK = KF ? b.fv[g] : nullptr;
+    int ord = 0;   // KF: done steps of the column not yet reached by the backward recursion
+    if constexpr (KF) {
+        if (FK)
+            for (int t = 0; t < T; t++) ord += b.done[(long long)t * E + e] != 0;
+    }
     const double gamma = b.gamma[g], gl = b.gl[g];
     int32_t dn[K], dnn[K];
     RT rn[K];
@@ -2081,7 +2090,11 @@ AIE_DEV void gae_column(const AdvantageBufs &b, int g, long long E, long long co
             const int t = hi - 1 - k;
             if (t < 0) break;
             const bool dk = d[k] != 0;
-            const double nv = dk ? (double)f[k] : (double)vnext;
+            double fk = (double)f[k];
+            if constexpr (KF) {
+                if (dk && FK) { --ord; fk = ord < nk ? (double)FK[(long long)ord * n + col] : (double)NAN; }
+            }
+            const double nv = dk ? fk : (double)vnext;
             const double delta = ((double)r[k] + gamma * nv) - (double)v[k];
             a = (dk || t == T - 1) ? delta : delta + gl * a;
             const long long i = (long long)t * n + col;

@@ -176,6 +176,7 @@ class BatchedFoundationEnv:
         self._world_dense_log_frequency = int(world_dense_log_frequency)
         assert self._world_dense_log_frequency >= 1
         self._dense_logger = None
+        self._rollout = None   # bind_rollout
         self._dense_log = {"world": [], "states": [], "actions": [], "rewards": []}
         self._last_ep_dense_log = dict(self._dense_log)
         self._auto_reset = bool(auto_reset)
@@ -501,7 +502,7 @@ class BatchedFoundationEnv:
 
     def _write_actions(self, actions):
         st = self._stepper
-        buf_a, buf_p = st.buf["actions_agent"], st.buf["actions_planner"]
+        buf_a, buf_p = self.action_buffers
         if actions is None:
             buf_a[...] = 0
             buf_p[...] = 0
@@ -545,6 +546,8 @@ class BatchedFoundationEnv:
             lg.before_step(st.to_numpy(st.buf["actions_agent"][0]), st.to_numpy(st.buf["actions_planner"][0])
                            if st.dims.n_act_planner else None)
         self._stepper.step()
+        if self._rollout is not None:
+            self._aim_rollout()
         if self._saez is not None:
             self._saez.after_step()
         if lg is not None:
@@ -561,7 +564,81 @@ class BatchedFoundationEnv:
 
     @property
     def action_buffers(self):
+        if self._rollout is not None:
+            return self._rollout.actions[min(self._stepper.rollout_slot, self._rollout.T - 1)]
         return self._stepper.buf["actions_agent"], self._stepper.buf["actions_planner"]
+
+    # ------------------------------------------------------------------ rollouts stored in place
+    def bind_rollout(self, T, final_obs=False):
+        """Store the next rollouts of T steps in place: returns a rollout object whose device tensors the kernels write
+        directly (include/aie_b200.h, aie_bind_rollout), so the loop copies nothing per step.
+
+        rollout.buf: every observation / mask tensor [T + 1, E, ...] (slot t: the observation step t's action is taken
+        from, slot T: the one after the last step), actions_agent / actions_planner [T, E, ...], reward [T, E, A + 1],
+        done [T, E]; with final_obs (needs auto_reset) final_<name> [K, E, ...], K = ceil(T / episode_length), row
+        (k, e) the observation of the state in which replica e's k-th episode end within the rollout ended.
+        rollout.obs[t] / rollout.final_obs[k] are the named views env.obs / env.final_obs build, rollout.rew[t] /
+        rollout.done[t] / rollout.actions[t] those of env.rew, env.done and env.action_buffers, all built here once.
+
+        While bound, with the slot cursor s (0 here and after restart_rollout()): env.obs / env.obs_tensors and
+        env.action_buffers show slot s (sample_actions writes there), env.rew / env.done the latest step's slot s - 1
+        (slot 0 before the first step), and step() advances s.  env.final_obs / env.final_obs_tensors are not written
+        while a rollout is bound (they keep what they held): the final observations go to rollout.final_obs.  reset() is allowed only at s == 0 and writes the first
+        observations into slot 0.  After T steps call restart_rollout(), which carries slot T into slot 0.
+        unbind_rollout() returns to the env's own buffers.  Dense logging (it reads replica 0's bound action, reward
+        and done buffers) is refused with a ValueError, a stepper_factory whose stepper cannot bind rollouts with
+        NotImplementedError."""
+        st = self._stepper
+        if not hasattr(st, "bind_rollout"):
+            raise NotImplementedError("this env's stepper cannot bind rollouts")
+        if self._create_dense_log_every is not None or self._dense_logger is not None:
+            raise ValueError("bind_rollout: dense logging reads the env's own action, reward and done buffers; "
+                             "construct the env without dense_log_frequency")
+        if final_obs and not self._auto_reset:
+            raise ValueError("final_obs=True needs auto_reset=True")
+        if self._rollout is not None:
+            raise ValueError("a rollout is already bound: unbind_rollout() first")
+        r = st.bind_rollout(T, final_obs=final_obs)
+        b, A = r.buf, self.n_agents
+        slot = lambda t: {k: b[k][t] for k in r.obs_names}
+        r.obs = [self._obs_views(slot(t)) for t in range(r.T + 1)]
+        r.obs_slots = [slot(t) for t in range(r.T + 1)]
+        r.final_obs = [self._obs_views({k: b["final_" + k][k_] for k in r.obs_names}) for k_ in range(r.K)] \
+            if final_obs else None
+        r.actions = [(b["actions_agent"][t], b["actions_planner"][t]) for t in range(r.T)]
+        if self.collate_agent_step_and_reset_data:
+            r.rew = [{"a": b["reward"][t][:, :A], "p": b["reward"][t][:, A]} for t in range(r.T)]
+        else:
+            r.rew = [dict({str(i): b["reward"][t][:, i] for i in range(A)}, p=b["reward"][t][:, A]) for t in range(r.T)]
+        r.done = [{"__all__": b["done"][t]} for t in range(r.T)]
+        self._rollout = r
+        self._aim_rollout()
+        return r
+
+    def restart_rollout(self):
+        """Start the next rollout in the bound tensors (after its T steps): slot T's observations move to slot 0."""
+        if self._rollout is None:
+            raise ValueError("no rollout bound")
+        self._stepper.restart_rollout()
+        self._aim_rollout()
+
+    def unbind_rollout(self):
+        """Back to the env's own buffers (env.obs, env.rew, ... as before bind_rollout)."""
+        if self._rollout is None:
+            return
+        self._stepper.unbind_rollout()
+        self._rollout = None
+        self._build_views()
+
+    @property
+    def rollout(self):
+        """The bound rollout object, or None."""
+        return self._rollout
+
+    def _aim_rollout(self):
+        r, s = self._rollout, self._stepper.rollout_slot
+        self.obs, self.obs_tensors = r.obs[s], r.obs_slots[s]
+        self.rew, self.done = r.rew[max(s - 1, 0)], r.done[max(s - 1, 0)]
 
     def sample_actions(self, logits_agent, logits_planner=None, *, seed, greedy=False, out=None):
         """A policy's actions, drawn on the device into `action_buffers` (then step(env.action_buffers) consumes them).
@@ -593,7 +670,8 @@ class BatchedFoundationEnv:
         action that is closed gives NaN (see include/aie_b200.h).  Asynchronous; the env's state is not touched."""
         return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
 
-    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0):
+    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0,
+                           per_episode_end=False):
         """Advantages and value targets of a stored rollout of T steps (generalised advantage estimation), bootstrapped
         at episode ends: (adv_agent [T, E, A], adv_planner [T, E], ret_agent, ret_planner), float32, one device launch.
 
@@ -607,8 +685,13 @@ class BatchedFoundationEnv:
         output over the whole final_obs tensor will do).  final_values=None treats an episode end as terminal.  gamma,
         lam: floats in [0, 1] or (agents, planner) pairs.  The planner entries may be None together (a trainer without
         a planner policy; its outputs are then None).  Computed in float64 exactly as include/aie_b200.h spells out.
-        Every tensor contiguous on the env's device; asynchronous on the current stream; the env's state is not touched."""
-        return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam)
+        Every tensor contiguous on the env's device; asynchronous on the current stream; the env's state is not touched.
+
+        A bound rollout's storage is taken as it is: rewards = rollout.buf["reward"] [T, E, A + 1] (split here with one
+        copy per group), dones = rollout.buf["done"], and with per_episode_end=True final_values [K, E, A] / [K, E], the
+        values of the final slots: a done step reads the row of its episode-end ordinal in its replica (0 for the first)."""
+        return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam,
+                                                per_episode_end=per_episode_end)
 
     # ------------------------------------------------------------------ outputs
     @staticmethod

@@ -280,6 +280,7 @@ class CovidBatchedEnv:
                                           % (self._obs_dtype, getattr(self._stepper, "obs_dtype", "float32")))
         self._final_obs = bool(final_obs)
         self._loaded = False
+        self._rollout = None   # bind_rollout
         self._build_views()
         self._build_rate_observation()
 
@@ -300,8 +301,97 @@ class CovidBatchedEnv:
 
     @property
     def action_buffers(self):
-        """(agent actions [E, S], planner actions [E]): write in place and call step(env.action_buffers) for zero copies."""
+        """(agent actions [E, S], planner actions [E]): write in place and call step(env.action_buffers) for zero copies.
+        With a rollout bound: slot s of its actions."""
+        if self._rollout is not None:
+            return self._rollout.actions[min(self._stepper.rollout_slot, self._rollout.T - 1)]
         return self._stepper.buf["actions_agent"], self._stepper.buf["actions_planner"]
+
+    # ------------------------------------------------------------------ rollouts stored in place
+    def bind_rollout(self, T, final_obs=False):
+        """Store the next rollouts of T steps in place (the contract of BatchedFoundationEnv.bind_rollout): rollout.buf
+        holds the seven observation / mask tensors [T + 1, E, ...], actions_agent [T, E, 51], actions_planner [T, E],
+        reward_agent [T, E, 51] float32, reward_planner [T, E] float64, done [T, E], and with final_obs (needs auto_reset)
+        final_<name> [K, E, ...], K = ceil(T / episode_length), written by the step kernel on the step that ends an
+        episode (every replica ends on the same step).  Under VaccinationCampaign(observe_rate=True) also
+        rate_agent [T + 1, E, 51] / rate_planner [T + 1, E] and final_rate_agent / final_rate_planner [K, ...]: the
+        next_vaccination_rate of each slot, from the same table lookup as env.obs.  rollout.obs[t] / rollout.final_obs[k]
+        are env.obs-style views, rollout.rew[t] / rollout.done[t] / rollout.actions[t] those of env.rew, env.done and
+        env.action_buffers.  While bound, env.obs and env.action_buffers show slot s, env.rew / env.done the latest
+        step's slot, step() advances s and reset() is allowed only at s == 0; env.final_obs is not written.  After T
+        steps, restart_rollout() carries slot T into slot 0.  A stepper_factory whose stepper cannot bind rollouts is
+        refused with NotImplementedError."""
+        st = self._stepper
+        if not hasattr(st, "bind_rollout"):
+            raise NotImplementedError("this env's stepper cannot bind rollouts")
+        if self._rollout is not None:
+            raise ValueError("a rollout is already bound: unbind_rollout() first")
+        r = st.bind_rollout(T, final_obs=final_obs)
+        b = r.buf
+        slot = lambda t: {k: b[k][t] for k in r.obs_names}
+        r.obs_slots = [slot(t) for t in range(r.T + 1)]
+        r.obs = [self._obs_views(r.obs_slots[t], "") for t in range(r.T + 1)]
+        r.final_obs = [self._obs_views({k: b["final_" + k][k_] for k in r.obs_names}, "") for k_ in range(r.K)] \
+            if final_obs else None
+        r.actions = [(b["actions_agent"][t], b["actions_planner"][t]) for t in range(r.T)]
+        r.rew = [{"a": b["reward_agent"][t], "p": b["reward_planner"][t]} for t in range(r.T)]
+        r.done = [{"__all__": b["done"][t]} for t in range(r.T)]
+        if self._rate_tab is not None:
+            E, S = self.n_envs, self.n_agents
+            zeros = (lambda sh: np.zeros(sh, self._rate_a.dtype)) if isinstance(self._rate_a, np.ndarray) else \
+                (lambda sh: self._rate_a.new_zeros(sh))
+            b["rate_agent"], b["rate_planner"] = zeros((r.T + 1, E, S)), zeros((r.T + 1, E))
+            for t in range(r.T + 1):
+                r.obs[t]["a"]["VaccinationCampaign-next_vaccination_rate"] = b["rate_agent"][t]
+                r.obs[t]["p"]["VaccinationCampaign-next_vaccination_rate"] = b["rate_planner"][t]
+            if final_obs:
+                b["final_rate_agent"], b["final_rate_planner"] = zeros((r.K, E, S)), zeros((r.K, E))
+                for k in range(r.K):
+                    r.final_obs[k]["a"]["VaccinationCampaign-next_vaccination_rate"] = b["final_rate_agent"][k]
+                    r.final_obs[k]["p"]["VaccinationCampaign-next_vaccination_rate"] = b["final_rate_planner"][k]
+        self._home_rate = (self._rate_a, self._rate_p) if self._rate_tab is not None else None
+        self._rollout = r
+        self._aim_rollout()
+        if self._loaded:
+            self._refresh_rate_observation()
+        return r
+
+    def restart_rollout(self):
+        """Start the next rollout in the bound tensors (after its T steps): slot T moves to slot 0."""
+        if self._rollout is None:
+            raise ValueError("no rollout bound")
+        self._stepper.restart_rollout()
+        r = self._rollout
+        if self._rate_tab is not None:
+            r.buf["rate_agent"][0][...] = r.buf["rate_agent"][r.T]
+            r.buf["rate_planner"][0][...] = r.buf["rate_planner"][r.T]
+        self._aim_rollout()
+
+    def unbind_rollout(self):
+        if self._rollout is None:
+            return
+        self._stepper.unbind_rollout()
+        self._rollout = None
+        if self._home_rate is not None:
+            self._rate_a, self._rate_p = self._home_rate
+        self._build_views()
+        if self._rate_tab is not None:
+            self.obs["a"]["VaccinationCampaign-next_vaccination_rate"] = self._rate_a
+            self.obs["p"]["VaccinationCampaign-next_vaccination_rate"] = self._rate_p
+            if self.final_obs is not None:
+                self.final_obs["a"]["VaccinationCampaign-next_vaccination_rate"] = self._final_rate_a
+                self.final_obs["p"]["VaccinationCampaign-next_vaccination_rate"] = self._final_rate_p
+
+    @property
+    def rollout(self):
+        return self._rollout
+
+    def _aim_rollout(self):
+        r, s = self._rollout, self._stepper.rollout_slot
+        self.obs = r.obs[s]
+        self.rew, self.done = r.rew[max(s - 1, 0)], r.done[max(s - 1, 0)]
+        if self._rate_tab is not None:
+            self._rate_a, self._rate_p = r.buf["rate_agent"][s], r.buf["rate_planner"][s]
 
     def sample_actions(self, logits_agent, logits_planner=None, *, seed, greedy=False, out=None):
         """A policy's actions, drawn on the device into `action_buffers` from the softmax of its logits restricted to the
@@ -319,13 +409,17 @@ class CovidBatchedEnv:
         [*B], entropy_agent [*B, 51], entropy_planner [*B]), differentiable with respect to both logits tensors."""
         return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
 
-    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0):
+    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0,
+                           per_episode_end=False):
         """Advantages and value targets of a stored rollout (the contract of BatchedFoundationEnv.compute_advantages),
         A = 51 states: rewards = (rew["a"] [T, E, 51] float32, rew["p"] [T, E] float64) stacked over the steps, values
         = (agent, planner) float32 of the same shapes, dones int32 [T, E], last_values = ([E, 51], [E]).  Every episode
         ends on its time limit, so it is truncated: final_values = the values of env.final_obs stored at each step
-        (env created with final_obs=True) bootstraps it; final_values=None treats an episode end as terminal."""
-        return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam)
+        (env created with final_obs=True) bootstraps it; final_values=None treats an episode end as terminal.  A bound
+        rollout: (rollout.buf["reward_agent"], rollout.buf["reward_planner"]), rollout.buf["done"] and, with
+        per_episode_end=True, the values of its [K, ...] final slots."""
+        return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam,
+                                                per_episode_end=per_episode_end)
 
     def _build_views(self):
         b = self._stepper.buf
@@ -397,7 +491,7 @@ class CovidBatchedEnv:
         """Each replica's timestep: from the float32 time scalar t / time_scale, which holds it exactly, or under bfloat16
         observations from hdr[:, 0] (a bfloat16 t / 540 spans one to two timesteps)."""
         b = self._stepper.buf
-        sc = b["obs_scalars"]
+        sc = b["obs_scalars"] if self._rollout is None else self._rollout.obs_slots[self._stepper.rollout_slot]["obs_scalars"]
         scale = float(self.params["time_scale"])
         if isinstance(sc, np.ndarray):
             return b["hdr"][:, 0] if sc.dtype == np.uint16 else np.rint(sc[:, 0].astype(np.float64) * scale).astype(np.int64)
@@ -417,7 +511,23 @@ class CovidBatchedEnv:
         else:
             self._rate_p.copy_(rate)
             self._rate_a.copy_(self._rate_p[:, None].expand_as(self._rate_a))
-        if stepped and self.final_obs is not None:
+        if stepped and self._rollout is not None:
+            r, s = self._rollout, self._stepper.rollout_slot
+            if r.final_obs is not None and s >= 1:
+                # the rows of the episodes this step ended, at their final slot k (the episode ends before it in the rollout)
+                done, last = r.buf["done"][s - 1] != 0, self._rate_tab[self._episode_length]
+                before = r.buf["done"][:s - 1].sum(0) if s > 1 else done * 0
+                fa, fp = r.buf["final_rate_agent"], r.buf["final_rate_planner"]
+                for k in range(r.K):
+                    m = done & (before == k)
+                    if isinstance(m, np.ndarray):
+                        fp[k][...] = np.where(m, last, fp[k])
+                        fa[k][...] = np.where(m[:, None], last, fa[k])
+                    else:
+                        import torch
+                        fp[k].copy_(torch.where(m, last, fp[k]))
+                        fa[k].copy_(torch.where(m[:, None], last, fa[k]))
+        elif stepped and self.final_obs is not None:
             # only the rows of the episodes this step ended
             done = b["done"] != 0
             last = self._rate_tab[self._episode_length]
@@ -432,13 +542,15 @@ class CovidBatchedEnv:
     def reset(self):
         self._stepper.reset()
         self._loaded = True
+        if self._rollout is not None:
+            self._aim_rollout()
         self._refresh_rate_observation()
         return self.obs
 
     def step(self, actions=None):
         """actions: None | {"a": int tensor [E, 51], "p": int tensor [E]} | (agent_actions, planner_actions)."""
         assert self._loaded, "call reset() first"
-        ba, bp = self._stepper.buf["actions_agent"], self._stepper.buf["actions_planner"]
+        ba, bp = self.action_buffers
         if actions is None:
             ba[...] = 0
             bp[...] = 0
@@ -455,6 +567,8 @@ class CovidBatchedEnv:
                         buf[...] = torch.as_tensor(np.asarray(v) if not isinstance(v, torch.Tensor) else v,
                                                    device=buf.device).to(buf.dtype).reshape(buf.shape)
         self._stepper.step()
+        if self._rollout is not None:
+            self._aim_rollout()
         self._refresh_rate_observation(stepped=True)
         return self.obs, self.rew, self.done, self.info
 

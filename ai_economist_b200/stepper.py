@@ -253,7 +253,8 @@ class PolicySampler:
             out.append(float(v))
         return out
 
-    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0):
+    def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0,
+                           per_episode_end=False):
         """Generalised advantage estimates and value targets of a stored rollout of T steps, bootstrapped at episode
         ends: (adv_agent, adv_planner, ret_agent, ret_planner), new float32 buffers shaped like the rewards.  rewards =
         (agent [T, E, A], planner [T, E]), float32 or float64 each; values = (agent, planner), float32 like the
@@ -264,6 +265,9 @@ class PolicySampler:
         state of the env is read or changed.  Anything else is a ValueError before the library is called."""
         sa = self._policy_shapes()[0]
         E, A = sa[0], sa[1]
+        if not isinstance(rewards, (tuple, list)) and tuple(getattr(rewards, "shape", ())[1:]) == (E, A + 1):
+            # a rollout's rewards as the env stores them, [T, E, A + 1] (agents, then the planner): split, one copy each
+            rewards = (self._contiguous(rewards[..., :A]), self._contiguous(rewards[..., A]))
         pairs = dict(rewards=rewards, values=values, last_values=last_values)
         if final_values is not None:
             pairs["final_values"] = final_values
@@ -281,6 +285,17 @@ class PolicySampler:
         if T > 0x7FFFFFFF:
             raise ValueError("T must fit in int32")
         rows = ((T, E, A), (T, E))
+        # final values [T, E, ...] (the row of each done step), or with per_episode_end=True [K, E, ...], K >= 1 (the row
+        # of each done step's episode-end ordinal in its column: a bound rollout's final slots, aie_compute_advantages_k)
+        K = None
+        if per_episode_end:
+            if final_values is None:
+                raise ValueError("per_episode_end=True needs final_values [K, E, ...]")
+            fs = tuple(getattr(final_values[0], "shape", ()))
+            if len(fs) != 3 or fs[1:] != (E, A) or fs[0] < 1:
+                raise ValueError("final_values[0] must be a [K, %d, %d] tensor, K >= 1, with per_episode_end=True" % (E, A))
+            K = fs[0]
+        frows = ((K or T, E, A), (K or T, E))
         rk = []
         for k, who in enumerate(("agent", "planner")[:2 if planner else 1]):
             kind = self._float_kind(rewards[k])
@@ -288,7 +303,7 @@ class PolicySampler:
                 raise ValueError("rewards[%d] (%s) must be a contiguous float32 or float64 %s tensor on the env's device"
                                  % (k, who, rows[k]))
             rk.append(kind)
-            for name, want in (("values", rows[k]), ("last_values", rows[k][1:]), ("final_values", rows[k])):
+            for name, want in (("values", rows[k]), ("last_values", rows[k][1:]), ("final_values", frows[k])):
                 if name in pairs and (self._float_kind(pairs[name][k]) != "f32" or tuple(pairs[name][k].shape) != want):
                     raise ValueError("%s[%d] (%s) must be a contiguous float32 %s tensor on the env's device"
                                      % (name, k, who, want))
@@ -313,8 +328,15 @@ class PolicySampler:
             q.final_values_agent = self._ptr(final_values[0])
             if planner:
                 q.final_values_planner = self._ptr(final_values[1])
-        self._check(self._adv_fn(self._h, C.byref(q), C.c_int32(T), self._stream()))
+        if K is not None:
+            self._check(self._adv_k_fn(self._h, C.byref(q), C.c_int32(T), C.c_int32(K), self._stream()))
+        else:
+            self._check(self._adv_fn(self._h, C.byref(q), C.c_int32(T), self._stream()))
         return adv_a, adv_p, ret_a, ret_p
+
+    @staticmethod
+    def _contiguous(x):
+        return x.contiguous() if hasattr(x, "contiguous") else np.ascontiguousarray(x)
 
     def _mask_rows(self):
         """(agent mask row, planner mask row or None): the logits' rows (COVID-19 overrides: its agent mask is transposed)."""
@@ -332,6 +354,28 @@ class PolicySampler:
 
     def _buf_kind(self, buf):
         return buf_kind_numpy(buf)
+
+
+class Rollout:
+    """The device tensors of a rollout of T steps stored in place (aie_bind_rollout), allocated by the stepper.
+
+    buf[name]: every observation / mask tensor [T + 1, E, ...] (slot t: the observation step t's action is taken from,
+    slot T: the one after the last step), "actions_agent" / "actions_planner" [T, E, ...], "reward" [T, E, A + 1] and
+    "done" [T, E] (step t's), and with final_obs "final_<name>" [K, E, ...], K = ceil(T / episode_length): row (k, e) the
+    observation of the state in which replica e's k-th episode end within the rollout ended."""
+
+    def __init__(self, T, K, buf, obs_names, final_obs):
+        self.T, self.K, self.buf = T, K, buf
+        self.obs_names = tuple(obs_names)
+        self.has_final_obs = final_obs
+
+    @property
+    def obs_tensors(self):
+        return {k: self.buf[k] for k in self.obs_names}
+
+    @property
+    def final_obs_tensors(self):
+        return {k: self.buf["final_" + k] for k in self.obs_names} if self.has_final_obs else None
 
 
 class BatchStepper(PolicySampler):
@@ -397,6 +441,9 @@ class BatchStepper(PolicySampler):
         if self.event_envs:
             shapes["events"] = ("i32", (self.event_envs, self.event_cap + 1, 8))
         self.buf = {k: self._alloc(shape, dt) for k, (dt, shape) in shapes.items()}
+        self._shapes = shapes
+        self.rollout = None   # the bound Rollout (bind_rollout), and its slot cursor
+        self.rollout_slot = 0
         self._bf16 = {k for k, (dt, _) in shapes.items() if dt == "bf16"}
         bufs = _abi.AieBuffers()
         for name in _abi._BUF_NAMES:
@@ -537,10 +584,50 @@ class BatchStepper(PolicySampler):
 
     def step(self):
         """Advance every env by one timestep from the bound action buffers (asynchronous on the stream); with final_obs,
-        then write the final observations of the episodes that ended into the final_<name> buffers."""
+        then write the final observations of the episodes that ended into the final_<name> buffers.  With a rollout
+        bound: from the actions of slot s into slot s (rewards, done) and s + 1 (observations), the final observations
+        into the rollout's final slots, then s advances."""
         self._check(self.lib.aie_step(self._h, self._stream()))
-        if self.final_obs:
+        if self.rollout is not None:
+            self.rollout_slot += 1
+        elif self.final_obs:
             self.observe_final()
+
+    # -- rollouts stored in place (aie_bind_rollout) ---------------------------------------------------------------
+    def bind_rollout(self, T, final_obs=False):
+        """Allocate and bind a rollout of T steps (a Rollout), with final slots [K, E, ...] when final_obs."""
+        if isinstance(T, bool) or not isinstance(T, numbers.Integral) or T < 1:
+            raise ValueError("T must be a positive int")
+        if self.rollout is not None:
+            raise ValueError("a rollout is already bound: unbind_rollout() first")
+        T = int(T)
+        K = -(-T // int(self.spec["episode_length"]))
+        sh = self._shapes
+        names = [k for k in _abi.OBS_NAMES if k in sh]
+        buf = {k: self._alloc((T + 1,) + sh[k][1], sh[k][0]) for k in names}
+        for k in ("actions_agent", "actions_planner", "reward", "done"):
+            buf[k] = self._alloc((T,) + sh[k][1], sh[k][0])
+        if final_obs:
+            buf.update({"final_" + k: self._alloc((K,) + sh[k][1], sh[k][0]) for k in names})
+        r = _abi.AieRollout()
+        r.T = T
+        r.obs = self._obs_buffers({k: buf[k] for k in names})
+        if final_obs:
+            r.final_obs = self._obs_buffers({k: buf["final_" + k] for k in names})
+        r.actions_agent, r.reward, r.done = self._ptr(buf["actions_agent"]), self._ptr(buf["reward"]), self._ptr(buf["done"])
+        r.actions_planner = self._ptr(buf["actions_planner"]) if self.dims.n_act_planner else None
+        self._check(self.lib.aie_bind_rollout(self._h, C.byref(r)))
+        self.rollout, self.rollout_slot = Rollout(T, K, buf, names, bool(final_obs)), 0
+        return self.rollout
+
+    def restart_rollout(self):
+        """Next rollout: the observations of slot T move to slot 0 (one device copy per tensor), s = 0."""
+        self._check(self.lib.aie_rollout_restart(self._h, self._stream()))
+        self.rollout_slot = 0
+
+    def unbind_rollout(self):
+        self._check(self.lib.aie_bind_rollout(self._h, None))
+        self.rollout, self.rollout_slot = None, 0
 
     def observe(self):
         self._check(self.lib.aie_observe(self._h, self._stream()))
@@ -603,6 +690,10 @@ class BatchStepper(PolicySampler):
     @property
     def _adv_fn(self):
         return self.lib.aie_compute_advantages
+
+    @property
+    def _adv_k_fn(self):
+        return self.lib.aie_compute_advantages_k
 
     def _policy_shapes(self):
         d, E, A = self.dims, self.n_envs, self.spec["n_agents"]

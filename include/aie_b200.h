@@ -506,6 +506,54 @@ typedef struct aie_advantage_args {
  * element size. */
 int aie_compute_advantages(aie_env *env, const aie_advantage_args *args, int32_t T, void *stream);
 
+/* Rollouts stored in place.  A rollout of T steps of the E replicas is a set of caller-owned DEVICE tensors, contiguous,
+ * slot-major: slot t of a tensor is the [E, ...] block of the bound buffer of the same name (aie_buffers), at
+ * t * (bytes of that block).  K = ceil(T / episode_length). */
+typedef struct aie_rollout {
+    int32_t T;                    /* slots of the step outputs, >= 1 */
+    aie_obs_buffers obs;          /* [T + 1, E, ...] each: slot t the observation step t's action is taken from, slot T the
+                                     observation after the last step (the bootstrap input).  NULL exactly where
+                                     aie_bind_buffers allows NULL */
+    int32_t *actions_agent;       /* [T, E, A, n_act_agent] */
+    int32_t *actions_planner;     /* [T, E, n_act_planner]; NULL when n_act_planner == 0 */
+    double *reward;               /* [T, E, A + 1] */
+    int32_t *done;                /* [T, E] */
+    aie_obs_buffers final_obs;    /* optional: every member NULL (no final slots), or [K, E, ...] each: row (k, e) the
+                                     observation of the state in which replica e's k-th episode end within this rollout
+                                     ended (k counts from 0).  Needs auto_reset and an episode_final buffer */
+} aie_rollout;
+
+/* ABI 6 (additive).  Binds a rollout: from here on the library keeps a slot cursor s (0 after this call) and
+ *   - aie_sample_random_actions / aie_sample_policy read the masks of slot s and write the actions into slot s;
+ *   - aie_step reads the actions of slot s, writes the observations and masks into slot s + 1 and the rewards and done
+ *     into slot s; with final slots it then writes the final observation of every episode it ended into row
+ *     (k, e) of final_obs, k = the number of done flags of replica e in slots 0 .. s - 1 (a replica ends at most K times
+ *     in T steps, since every episode lasts episode_length steps; a k >= K is not written); then s advances.  With final
+ *     slots that is two launches (the step, then the final pass: the same count as aie_step + aie_observe_final today),
+ *     without them one;
+ *   - aie_observe writes the observations of the current state into slot s;
+ *   - aie_load_state / aie_reset_envs write the first observations into slot 0, and are allowed only at s == 0.
+ * AIE_ESTATE while a rollout is bound: aie_step, the samplers at s == T; aie_load_state / aie_reset_envs at s != 0;
+ * aie_set_fused_policy (its draws would overwrite the stored actions), aie_step_dynamics, aie_observe_final (the final
+ * slots replace it), aie_step_host, aie_step_host_compact and aie_bind_buffers.  s advances once the step launch succeeds (the state
+ * has then moved on), even if the final pass after it fails; any other call that fails leaves s where it was.
+ * r == NULL unbinds: every pointer returns to the buffers of aie_bind_buffers, so a caller that never binds a rollout sees
+ * no change.  No launch; no device work.  AIE_EINVAL for T < 1, a NULL required pointer, a pointer not aligned to its
+ * element size, or final slots partly given; AIE_ESTATE before aie_bind_buffers, with the fused random policy on, or
+ * final slots without auto_reset and an episode_final buffer. */
+int aie_bind_rollout(aie_env *env, const aie_rollout *r);
+/* Starts the next rollout of the bound tensors: copies the observations of slot T into slot 0 (one device copy per
+ * tensor), sets s = 0 and so restarts the episode-end count k.  Asynchronous on `stream`; no launch.  AIE_ESTATE without
+ * a bound rollout or before its T steps are done (s != T). */
+int aie_rollout_restart(aie_env *env, void *stream);
+/* The advantages of aie_compute_advantages over a bound rollout's final slots: final_values_* are [K, E, A] / [K, E]
+ * (the value of final_obs row (k, e)), and a done step reads the row of its episode-end ordinal within the column
+ * (0 for the first done flag of replica e in 0 .. T-1); an ordinal >= K reads NaN.  Every other input, the recursion,
+ * its rounding and its NaN behaviour are aie_compute_advantages's, so the result has the same bits as that call over
+ * [T, E, ...] final values holding row (k, e) at the k-th done step of replica e.  One launch.  AIE_EINVAL as
+ * aie_compute_advantages, and for K < 1. */
+int aie_compute_advantages_k(aie_env *env, const aie_advantage_args *args, int32_t T, int32_t K, void *stream);
+
 /* End-to-end variant with HOST buffers: copies the actions host->device, steps, copies every non-NULL
  * output device->host, and synchronises the stream.  Buffers should be pinned for full PCIe rate. */
 int aie_step_host(aie_env *env, const int32_t *actions_agent_host, const int32_t *actions_planner_host,
@@ -677,6 +725,36 @@ int aie_covid_evaluate_policy_backward(aie_covid_env *env, const aie_policy_eval
 /* Advantages and value targets of a stored rollout (the contract of aie_compute_advantages), A = S states. */
 int aie_covid_compute_advantages(aie_covid_env *env, const aie_advantage_args *args, int32_t T, void *stream);
 int64_t aie_covid_launch_count(const aie_covid_env *env);
+
+/* A COVID-19 rollout stored in place (the contract of aie_rollout, with this scenario's tensors); K = ceil(T /
+ * episode_length). */
+typedef struct aie_covid_rollout {
+    int32_t T;                    /* >= 1 */
+    aie_covid_obs_buffers obs;    /* [T + 1, E, ...] each (slot t: the observation step t's action is taken from) */
+    int32_t *actions_agent;       /* [T, E, S] */
+    int32_t *actions_planner;     /* [T, E] */
+    float *reward_agent;          /* [T, E, S] */
+    double *reward_planner;       /* [T, E] */
+    int32_t *done;                /* [T, E] */
+    aie_covid_obs_buffers final_obs;   /* optional (every member NULL: none): [K, E, ...] each, row (k, e) the observation of
+                                          the state in which replica e's k-th episode end within the rollout ended */
+} aie_covid_rollout;
+/* ABI 6 (additive).  aie_bind_rollout for the COVID-19 scenario: while bound, the samplers read the masks of slot s and
+ * write the actions into slot s; aie_covid_step reads the actions of slot s, writes the observations into slot s + 1 and
+ * the rewards and done into slot s, and on the step that ends an episode writes its final observations into row (k, e)
+ * of final_obs in the same launch (aie_covid_step_final's kernel with its destination moved to row k); then s advances.
+ * Every replica ends on the same step: aie_covid_reset starts them all at t = 0 and they step in lock-step, so k is one
+ * host-side count (the episode ends this rollout has seen; hdr[:, 3], the episodes counter, grows by one on each) and
+ * the step kernels are unchanged.  A caller that writes hdr's t itself breaks the lock-step and must not bind final
+ * slots.  aie_covid_reset writes into slot 0 and is allowed only at s == 0.  AIE_ESTATE while bound: aie_covid_step and
+ * the samplers at s == T, aie_covid_reset at s != 0, aie_covid_step_final and aie_covid_bind_buffers.  r == NULL
+ * unbinds.  No launch.  AIE_EINVAL for T < 1, a NULL required pointer, a pointer not aligned to its element, or final
+ * slots partly given; AIE_ESTATE before aie_covid_bind_buffers, or final slots without auto_reset. */
+int aie_covid_bind_rollout(aie_covid_env *env, const aie_covid_rollout *r);
+/* aie_rollout_restart for the COVID-19 scenario. */
+int aie_covid_rollout_restart(aie_covid_env *env, void *stream);
+/* aie_compute_advantages_k for the COVID-19 scenario, A = S states. */
+int aie_covid_compute_advantages_k(aie_covid_env *env, const aie_advantage_args *args, int32_t T, int32_t K, void *stream);
 
 const char *aie_last_error(void);
 int aie_abi_version(void);
