@@ -188,6 +188,16 @@ class AieCovidObsBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in COVID_OBS_NAMES]
 
 
+class AieCovidMetricBuffers(C.Structure):
+    """aie_covid_metric_buffers: the episode-metric accumulators of a COVID-19 env (aie_covid_bind_metrics)."""
+    _fields_ = [("sums", C.c_void_p), ("prev_sums", C.c_void_p), ("index", C.c_void_p), ("prev_index", C.c_void_p),
+                ("prev_end", C.c_void_p), ("us_population", C.c_double)]
+
+
+class AieCovidMetricColumn(C.Structure):
+    _fields_ = [("state", C.c_int32), ("field", C.c_char * 60)]
+
+
 class AieCovidRollout(C.Structure):
     """aie_covid_rollout: the device tensors of a COVID-19 rollout stored in place (aie_covid_bind_rollout)."""
     _fields_ = [("T", C.c_int32), ("obs", AieCovidObsBuffers), ("actions_agent", C.c_void_p),
@@ -250,6 +260,12 @@ def load_library(path=None):
     L.aie_covid_bind_rollout.restype = C.c_int
     L.aie_covid_rollout_restart.argtypes = [P, P]
     L.aie_covid_rollout_restart.restype = C.c_int
+    L.aie_covid_bind_metrics.argtypes = [P, C.POINTER(AieCovidMetricBuffers)]
+    L.aie_covid_bind_metrics.restype = C.c_int
+    L.aie_covid_get_metric_layout.argtypes = [P, C.POINTER(AieCovidMetricColumn), C.c_int32]
+    L.aie_covid_get_metric_layout.restype = C.c_int
+    L.aie_covid_episode_metrics.argtypes = [P, C.c_int32, P, P]
+    L.aie_covid_episode_metrics.restype = C.c_int
     L.aie_step_host.argtypes = [P, P, P, C.POINTER(AieHostOut), P]
     L.aie_step_host_compact.argtypes = [P, P, P, C.POINTER(AieHostOut), C.c_int32, P]
     L.aie_step_host_compact.restype = C.c_int
@@ -294,7 +310,8 @@ EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field"
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
                     "aie_covid_step_final", "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
                     "aie_covid_evaluate_policy_backward", "aie_covid_compute_advantages", "aie_covid_launch_count",
-                    "aie_covid_bind_rollout", "aie_covid_rollout_restart", "aie_covid_compute_advantages_k"]
+                    "aie_covid_bind_rollout", "aie_covid_rollout_restart", "aie_covid_compute_advantages_k",
+                    "aie_covid_bind_metrics", "aie_covid_get_metric_layout", "aie_covid_episode_metrics"]
 
 
 def obs_dtype_name(obs_dtype):

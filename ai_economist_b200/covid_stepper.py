@@ -76,7 +76,7 @@ class CovidStepperBase(PolicySampler):
     _DT = {"f32": np.float32, "f64": np.float64, "i32": np.int32, "i8": np.int8, "bf16": np.uint16}
 
     def __init__(self, params, n_envs, lib, device_index=0, auto_reset=True, change_list=None, final_obs=False,
-                 obs_dtype=None):
+                 obs_dtype=None, episode_metrics=False):
         # obs_dtype: element type of the seven observation / mask buffers (and their final_ twins), float32 (default)
         # or bfloat16, each element the round-to-nearest-even of the float32 a float32 env writes.
         self.obs_dtype = _abi.obs_dtype_name(obs_dtype)
@@ -126,6 +126,19 @@ class CovidStepperBase(PolicySampler):
             for name in _abi.COVID_OBS_NAMES:
                 self.buf["final_" + name] = self._alloc(shapes[name][1], shapes[name][0])
                 setattr(self._final_bufs, name, self._ptr(self.buf["final_" + name]))
+        # episode_metrics: keep the episode-metric accumulators (aie_covid_bind_metrics); the step kernels add to them
+        # and episode_metrics() turns them into scenario_metrics() rows.  Bound before the first reset, which zeroes them.
+        self.episode_metrics_on = bool(episode_metrics)
+        self._auto_reset, self._t, self._ended = bool(auto_reset), 0, False   # host mirror of the lock-step timestep
+        if self.episode_metrics_on:
+            m = _abi.AieCovidMetricBuffers()
+            for name, dt, shape in [("sums", "f64", (E, 4, S)), ("prev_sums", "f64", (E, 4, S)),
+                                    ("index", "f32", (E, 2, S + 1)), ("prev_index", "f32", (E, 2, S + 1)),
+                                    ("prev_end", "f32", (E, 4, S))]:
+                self.buf["metric_" + name] = self._alloc(shape, dt)
+                setattr(m, name, self._ptr(self.buf["metric_" + name]))
+            m.us_population = float(params["us_population"])
+            self._check(lib.aie_covid_bind_metrics(self._h, C.byref(m)))
 
     def _check(self, rc):
         if rc != _abi.AIE_OK:
@@ -147,6 +160,16 @@ class CovidStepperBase(PolicySampler):
 
     def reset(self):
         self._check(self.lib.aie_covid_reset(self._h, self._stream()))
+        self._t = 0
+
+    def _stepped(self):
+        self._t += 1
+        if self._auto_reset and self._t >= int(self.p["episode_length"]):
+            self._t, self._ended = 0, True
+
+    def has_previous_episode(self):
+        """Whether an episode has ended under the auto-reset (every replica ends on the same step)."""
+        return self._ended
 
     def step(self):
         if self.rollout is not None:   # slot s -> s + 1; the final observations go to the rollout's final slots
@@ -156,6 +179,7 @@ class CovidStepperBase(PolicySampler):
             self._check(self.lib.aie_covid_step_final(self._h, C.byref(self._final_bufs), self._stream()))
         else:
             self._check(self.lib.aie_covid_step(self._h, self._stream()))
+        self._stepped()
 
     # -- rollouts stored in place (aie_covid_bind_rollout) -----------------------------------------------------------
     def bind_rollout(self, T, final_obs=False):
@@ -224,6 +248,33 @@ class CovidStepperBase(PolicySampler):
     def launch_count(self):
         return int(self.lib.aie_covid_launch_count(self._h))
 
+    # -- episode metrics (aie_covid_bind_metrics / aie_covid_episode_metrics) -------------------------------------------
+    def metric_layout(self):
+        """[(key, is_int)] of the metric columns: "<state name>/<field>" for each state, then "usa/<field>" (the
+        reference's scenario_metrics() keys in its dict order); no column is an int."""
+        if getattr(self, "_metric_layout", None) is None:
+            n = self.lib.aie_covid_get_metric_layout(self._h, None, 0)
+            if n < 0:
+                self._check(n)
+            arr = (_abi.AieCovidMetricColumn * n)()
+            self.lib.aie_covid_get_metric_layout(self._h, arr, n)
+            names = self.p["state_names"]
+            self._metric_layout = [("%s/%s" % ("usa" if arr[i].state < 0 else names[arr[i].state], arr[i].field.decode()),
+                                    False) for i in range(n)]
+        return list(self._metric_layout)
+
+    def episode_metrics(self, final=False, out=None):
+        """scenario_metrics() of every replica as float64 [n_envs, K] in metric_layout() order, one launch, asynchronous
+        (aie_covid_episode_metrics).  final=True: of the episode each replica finished last.  out: an optional contiguous
+        float64 [n_envs, K] buffer of this stepper's kind."""
+        K = len(self.metric_layout())
+        if out is None:
+            out = self._alloc((self.n_envs, K), "f64")
+        elif self._float_kind(out) != "f64" or tuple(out.shape) != (self.n_envs, K):
+            raise _abi.AieError("episode_metrics: out must be a contiguous float64 [%d, %d] buffer" % (self.n_envs, K))
+        self._check(self.lib.aie_covid_episode_metrics(self._h, 1 if final else 0, self._ptr(out), self._stream()))
+        return out
+
     def obs_to_numpy(self, name, e=None):
         """Host copy of buffer `name` (of env e), bfloat16 observations as float32 (exact: every bfloat16 is a float32)."""
         a = self.to_numpy(self.buf[name] if e is None else self.buf[name][e])
@@ -247,7 +298,7 @@ class CovidStepperBase(PolicySampler):
 
 class CudaCovidStepper(CovidStepperBase):
     def __init__(self, params, n_envs, device="cuda:0", auto_reset=True, lib_path=None, change_list=None, final_obs=False,
-                 obs_dtype=None):
+                 obs_dtype=None, episode_metrics=False):
         import torch
 
         if not torch.cuda.is_available():
@@ -259,7 +310,7 @@ class CudaCovidStepper(CovidStepperBase):
         lib = _abi.load_library(lib_path)
         with torch.cuda.device(self.device):
             super().__init__(params, n_envs, lib, device_index=idx, auto_reset=auto_reset, change_list=change_list,
-                             final_obs=final_obs, obs_dtype=obs_dtype)
+                             final_obs=final_obs, obs_dtype=obs_dtype, episode_metrics=episode_metrics)
 
     def _alloc(self, shape, dt):
         t = self.torch

@@ -28,6 +28,11 @@
 //   aie_covid_{reset,step,step_final,sample}_bf16_kernel, aie_covid_sample_policy_kernel<LT, bf16_t>  the COVID-19
 //                          kernels over bfloat16 observations and masks (aie_covid_config::obs_dtype == AIE_OBS_BF16),
 //                          with their float32 twins' launch shapes.
+//   aie_covid_{reset,step,step_final}_stats_kernel<OT>  the COVID-19 reset and step kernels of an env with metric
+//                          buffers bound (aie_covid_bind_metrics), float32 or bfloat16 observations: the same bodies,
+//                          which also zero / accumulate the episode-metric sums.
+//   aie_covid_metrics_kernel  one CTA per env, one thread per state: a row of scenario_metrics() from the accumulators
+//                          and the state (aie_covid_episode_metrics).
 //   aie_compute_advantages_kernel  one thread per column of a stored rollout (agent and planner columns, group-uniform
 //                          CTAs): advantages and value targets (aie_compute_advantages, aie_covid_compute_advantages).
 //   aie_observe_final_slot_kernel  aie_observe_final_kernel's shape and body, writing into a bound rollout's final slots:
@@ -119,6 +124,7 @@ int covid_launch_reset(aie_covid_env *, void *stream);
 int covid_launch_step(aie_covid_env *, void *stream);
 int covid_launch_step_final(aie_covid_env *, const CovidBufs &fin, void *stream);
 int covid_launch_sample(aie_covid_env *, uint64_t key, void *stream);
+int covid_launch_metrics(aie_covid_env *, int source, double *out, void *stream);
 int covid_launch_policy(aie_covid_env *, const PolicyBufs &p, int lt_bf16, uint64_t sd, void *stream);
 int launch_policy_eval(aie_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows, void *stream);
 int covid_launch_policy_eval(aie_covid_env *, const PolicyEvalBufs &p, int mt_bf16, int lt_bf16, int bwd, long long n_rows,
@@ -1087,6 +1093,34 @@ __global__ void __launch_bounds__(64) aie_covid_sample_bf16_kernel(const __grid_
                                                                    uint64_t key) {
     covid_sample_env<bf16_t>(c, blockIdx.x, b, cv_mix64(key ^ cv_mix64(blockIdx.x)), threadIdx.x, blockDim.x);
 }
+// *_stats: the kernels an env with metric buffers bound launches (aie_covid_bind_metrics): the same bodies, which also
+// accumulate the episode metrics into m (covid_step_env's STATS) or zero its current block (reset).  OT: the element
+// type of the observation / mask tensors.
+template <typename OT>
+__global__ void __launch_bounds__(64) aie_covid_step_stats_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                  const __grid_constant__ CovidStats m) {
+    __shared__ float red[3 * 64];
+    __shared__ uint32_t chg[64 * CV_CHG_CAP];
+    covid_step_env<false, OT, true>(c, blockIdx.x, b, b, red, chg, threadIdx.x, blockDim.x, &m);
+}
+template <typename OT>
+__global__ void __launch_bounds__(64) aie_covid_step_final_stats_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                        const CovidBufs fin, const __grid_constant__ CovidStats m) {
+    __shared__ float red[3 * 64];
+    __shared__ uint32_t chg[64 * CV_CHG_CAP];
+    covid_step_env<true, OT, true>(c, blockIdx.x, b, fin, red, chg, threadIdx.x, blockDim.x, &m);
+}
+template <typename OT>
+__global__ void __launch_bounds__(64) aie_covid_reset_stats_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                   const __grid_constant__ CovidStats m) {
+    covid_reset_env<OT>(c, blockIdx.x, b, threadIdx.x, blockDim.x, false);
+    covid_zero_stats(c, blockIdx.x, m, threadIdx.x, blockDim.x);
+}
+// aie_covid_episode_metrics: one CTA per replica, one thread per state; thread 0 also forms the USA columns.
+__global__ void __launch_bounds__(64) aie_covid_metrics_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                               const __grid_constant__ CovidStats m, int source, double *out) {
+    covid_metrics_env(c, blockIdx.x, b, m, source, out, threadIdx.x, blockDim.x);
+}
 // Policy sampler (aie_covid_sample_policy): one warp per (env, unit), units = S states + the planner, eight per CTA.
 // LT: the logits' element type; MT: the masks' (bf16_t for a bfloat16 env).
 template <typename LT, typename MT>
@@ -1143,7 +1177,11 @@ void *dev_alloc(size_t bytes) {
 }
 void const_free(void *dev) { cudaFree(dev); }
 int covid_launch_reset(aie_covid_env *env, void *stream) {
-    if (env->obs_bf16) aie_covid_reset_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (env->metrics_on) {
+        if (env->obs_bf16) aie_covid_reset_stats_kernel<bf16_t><<<env->n_envs, 64, 0, st>>>(env->cfg, env->bufs, env->stats);
+        else aie_covid_reset_stats_kernel<float><<<env->n_envs, 64, 0, st>>>(env->cfg, env->bufs, env->stats);
+    } else if (env->obs_bf16) aie_covid_reset_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     else aie_covid_reset_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     AIE_CUDA(cudaGetLastError(), "aie_covid_reset_kernel launch");
     env->launches++;
@@ -1187,16 +1225,30 @@ int covid_launch_policy_eval(aie_covid_env *env, const PolicyEvalBufs &p, int mt
     return AIE_OK;
 }
 int covid_launch_step(aie_covid_env *env, void *stream) {
-    if (env->obs_bf16) aie_covid_step_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (env->metrics_on) {
+        if (env->obs_bf16) aie_covid_step_stats_kernel<bf16_t><<<env->n_envs, 64, 0, st>>>(env->cfg, env->bufs, env->stats);
+        else aie_covid_step_stats_kernel<float><<<env->n_envs, 64, 0, st>>>(env->cfg, env->bufs, env->stats);
+    } else if (env->obs_bf16) aie_covid_step_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     else aie_covid_step_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs);
     AIE_CUDA(cudaGetLastError(), "aie_covid_step_kernel launch");
     env->launches++;
     return AIE_OK;
 }
 int covid_launch_step_final(aie_covid_env *env, const CovidBufs &fin, void *stream) {
-    if (env->obs_bf16) aie_covid_step_final_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, fin);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (env->metrics_on) {
+        if (env->obs_bf16) aie_covid_step_final_stats_kernel<bf16_t><<<env->n_envs, 64, 0, st>>>(env->cfg, env->bufs, fin, env->stats);
+        else aie_covid_step_final_stats_kernel<float><<<env->n_envs, 64, 0, st>>>(env->cfg, env->bufs, fin, env->stats);
+    } else if (env->obs_bf16) aie_covid_step_final_bf16_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, fin);
     else aie_covid_step_final_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, fin);
     AIE_CUDA(cudaGetLastError(), "aie_covid_step_final_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+int covid_launch_metrics(aie_covid_env *env, int source, double *out, void *stream) {
+    aie_covid_metrics_kernel<<<env->n_envs, 64, 0, (cudaStream_t)stream>>>(env->cfg, env->bufs, env->stats, source, out);
+    AIE_CUDA(cudaGetLastError(), "aie_covid_metrics_kernel launch");
     env->launches++;
     return AIE_OK;
 }

@@ -60,6 +60,21 @@ constexpr uint32_t CV_LIST_DAY0 = 1u << 20;
 enum { CVS_S = 0, CVS_I, CVS_R, CVS_D, CVS_V, CVS_U, CVS_STRG, CVS_SUBSIDY, CVS_POST, CVS_FIELDS = 9 };
 enum { CVH_T = 0, CVH_SUBSIDY_LEVEL, CVH_RING_HEAD, CVH_EPISODES };
 
+// Episode-metric accumulators (aie_covid_bind_metrics), caller-owned, two blocks per replica:
+//   sums  float64 [E][CVM_SUMS][S]: sums over t = 1..t of the float32 Unemployed, Stringency Level, Postsubsidy
+//         Productivity and Subsidy the step stores (the reference's global_state[...][1:] time aggregates)
+//   index float32 [E][2][S + 1]: Health Index, Economic Index of each state, then the planner's, summed as the reference
+//         sums them (covid19_env.py:1124-1125, 1160-1161)
+//   end   float32 [E][4][S] (previous block only): I, R, D, V of the state the episode ended in
+// The current block is zeroed by aie_covid_reset and by the step that ends an episode, after copying it to the previous.
+enum { CVM_U = 0, CVM_STRG, CVM_POST, CVM_SUBSIDY, CVM_SUMS = 4 };
+constexpr int CVM_PER_STATE = 8, CVM_USA = 7;   // metric columns: 8 per state, then 7 for the USA
+struct CovidStats {
+    double *sums, *prev_sums;
+    float *index, *prev_index, *prev_end;
+    double us_pop;
+};
+
 #if CV_ON_DEVICE
 CV_DEV void cv_bsync() { __syncthreads(); }
 #else
@@ -220,9 +235,13 @@ constexpr int CV_CHG_CAP = 32;
 // FINAL: on the step that ends an episode under the auto-reset, first write the observations / masks of the state the
 // episode ended in into row e of fin's seven observation / mask tensors (fin: b with those pointers replaced), then
 // reset.  Unused without FINAL.  OT: the element type of the observation / mask tensors (covid_observe).
-template <bool FINAL, typename OT = float>
+// STATS: add this step's values to the current block of *ms (CovidStats); on the step that ends an episode under the
+// auto-reset, write the sums with this step's values to the previous block, with the end state, and zero the current
+// one.  Each state's thread owns its columns and thread 0 the planner's, so no reduction across states.  ms is unused
+// without STATS.
+template <bool FINAL, typename OT = float, bool STATS = false>
 CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const CovidBufs &fin, float *red, uint32_t *chg,
-                           int tid, int nthr) {
+                           int tid, int nthr, const CovidStats *ms = nullptr) {
     const int S = c.S, L = c.L, L1 = c.L + 1, F = c.F;
     float *st = b.state + (size_t)e * CVS_FIELDS * S;
     int32_t *ints = b.ints + (size_t)e * 2 * S;
@@ -388,6 +407,25 @@ CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const C
         const float wh = c.w_ah[a], we = c.w_ae[a];
             b.rew_a[(size_t)e * S + a] = (((wh * h) + (we * ec)) / (wh + we)) / (float)c.reward_norm;
         red_md[a] = md; red_sub[a] = subsidy; red_post[a] = post;
+        if (STATS) {
+            double *cs = ms->sums + (size_t)e * CVM_SUMS * S + a;
+            float *ci = ms->index + (size_t)e * 2 * (S + 1) + a;
+            const double su = cs[CVM_U * S] + (double)(float)unemployed, sg = cs[CVM_STRG * S] + (double)strg;
+            const double sp = cs[CVM_POST * S] + (double)post, ss = cs[CVM_SUBSIDY * S] + (double)subsidy;
+            const float ih = ci[0] + h, ie = ci[S + 1] + ec;
+            if (c.auto_reset && t >= c.T) {
+                double *ps = ms->prev_sums + (size_t)e * CVM_SUMS * S + a;
+                float *pi = ms->prev_index + (size_t)e * 2 * (S + 1) + a, *pe = ms->prev_end + (size_t)e * 4 * S + a;
+                ps[CVM_U * S] = su; ps[CVM_STRG * S] = sg; ps[CVM_POST * S] = sp; ps[CVM_SUBSIDY * S] = ss;
+                pi[0] = ih; pi[S + 1] = ie;
+                pe[0] = I_t; pe[S] = R_t; pe[2 * S] = D_t; pe[3 * S] = V_t;
+                cs[CVM_U * S] = 0.0; cs[CVM_STRG * S] = 0.0; cs[CVM_POST * S] = 0.0; cs[CVM_SUBSIDY * S] = 0.0;
+                ci[0] = 0.0f; ci[S + 1] = 0.0f;
+            } else {
+                cs[CVM_U * S] = su; cs[CVM_STRG * S] = sg; cs[CVM_POST * S] = sp; cs[CVM_SUBSIDY * S] = ss;
+                ci[0] = ih; ci[S + 1] = ie;
+            }
+        }
     }
     cv_bsync();
     if (tid == 0) {
@@ -400,6 +438,17 @@ CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const C
         pe = cv_minmax(pe, c.min_pe, c.max_pe);
         const double num = (double)c.w_ph * ph + (double)(c.w_pe * pe);
         b.rew_p[e] = (num / (double)(c.w_ph + c.w_pe)) / c.reward_norm;
+        if (STATS) {   // the planner's float32 indices; ph is float64 there (covid19_env.py:1160-1161)
+            float *ci = ms->index + (size_t)e * 2 * (S + 1);
+            const float ih = (float)((double)ci[S] + ph), ie = ci[2 * S + 1] + pe;
+            if (c.auto_reset && t >= c.T) {
+                float *pi = ms->prev_index + (size_t)e * 2 * (S + 1);
+                pi[S] = ih; pi[2 * S + 1] = ie;
+                ci[S] = 0.0f; ci[2 * S + 1] = 0.0f;
+            } else {
+                ci[S] = ih; ci[2 * S + 1] = ie;
+            }
+        }
         b.done[e] = t >= c.T ? 1 : 0;
         hdr[CVH_T] = t; hdr[CVH_SUBSIDY_LEVEL] = level; hdr[CVH_RING_HEAD] = new_head;
     }
@@ -420,6 +469,60 @@ CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const C
 // The step without final observations (aie_covid_step).
 CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, float *red, uint32_t *chg, int tid, int nthr) {
     covid_step_env<false>(c, e, b, b, red, chg, tid, nthr);
+}
+
+// aie_covid_reset with metrics bound: the current block starts from zero.
+CV_DEV void covid_zero_stats(const CovidCfg &c, int e, const CovidStats &ms, int tid, int nthr) {
+    const int S = c.S;
+    for (int i = tid; i < CVM_SUMS * S; i += nthr) ms.sums[(size_t)e * CVM_SUMS * S + i] = 0.0;
+    for (int i = tid; i < 2 * (S + 1); i += nthr) ms.index[(size_t)e * 2 * (S + 1) + i] = 0.0f;
+}
+
+// One row of aie_covid_episode_metrics: CovidAndEconomySimulation.scenario_metrics() (covid19_env.py:1613-1687) from an
+// end state `end` (float32 [4][S]: I, R, D, V), the time sums `sums` ([CVM_SUMS][S]) and the indices `index`
+// ([2][S + 1]).  Columns: 8 per state (CVM_PER_STATE), then the 7 USA columns.  Means over time divide by
+// episode_length (the reference's global_state rows 1..episode_length, zero after t).  Every value is one float64
+// expression in a fixed order; the USA sums run over the states in index order on thread 0.
+CV_DEV void covid_metrics_row(const CovidCfg &c, const float *end, const double *sums, const float *index, double us_pop,
+                              double *row, int tid, int nthr) {
+    const int S = c.S;
+    const double T = (double)c.T;
+    for (int a = tid; a < S; a += nthr) {
+        double *r = row + (size_t)a * CVM_PER_STATE;
+        r[0] = (double)(int32_t)end[a] / 1e6;           // Total Infected / Recovered / Deaths: int32 casts
+        r[1] = (double)(int32_t)end[S + a] / 1e6;
+        r[2] = (double)(int32_t)end[2 * S + a] / 1e6;
+        r[3] = ((sums[CVM_U * S + a] / T) / (double)c.pop[a]) * 100.0;
+        r[4] = sums[CVM_STRG * S + a] / T;
+        r[5] = sums[CVM_POST * S + a] / 1e9;
+        r[6] = (double)index[a];
+        r[7] = (double)index[S + 1 + a];
+    }
+    if (tid == 0) {
+        double v = 0.0, d = 0.0, u = 0.0, sub = 0.0, post = 0.0;
+        for (int a = 0; a < S; a++) {
+            v += (double)end[3 * S + a]; d += (double)end[2 * S + a];
+            u += sums[CVM_U * S + a]; sub += sums[CVM_SUBSIDY * S + a]; post += sums[CVM_POST * S + a];
+        }
+        double *r = row + (size_t)S * CVM_PER_STATE;
+        r[0] = (v / us_pop) * 100.0;
+        r[1] = d / 1e3;
+        r[2] = ((u / us_pop) / T) * 100.0;
+        r[3] = sub / 1e12;
+        r[4] = post / 1e12;
+        r[5] = (double)index[S];
+        r[6] = (double)index[2 * S + 1];
+    }
+}
+// source 0: the current block and the live state of replica e; 1: the previous block and its end state
+CV_DEV void covid_metrics_env(const CovidCfg &c, int e, const CovidBufs &b, const CovidStats &ms, int source, double *out,
+                              int tid, int nthr) {
+    const int S = c.S;
+    const size_t K = (size_t)S * CVM_PER_STATE + CVM_USA;
+    const float *end = source ? ms.prev_end + (size_t)e * 4 * S : b.state + (size_t)e * CVS_FIELDS * S + CVS_I * S;
+    const double *sums = (source ? ms.prev_sums : ms.sums) + (size_t)e * CVM_SUMS * S;
+    const float *index = (source ? ms.prev_index : ms.index) + (size_t)e * 2 * (S + 1);
+    covid_metrics_row(c, end, sums, index, ms.us_pop, out + (size_t)e * K, tid, nthr);
 }
 
 // Random policy: uniform over the unmasked actions (NO-OP is always open).

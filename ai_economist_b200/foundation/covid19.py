@@ -42,6 +42,9 @@ def build_covid_params(episode_length=540, start_date="2020-03-22", pop_between_
     S = len(pop)
     p["n_states"] = S
     p["episode_length"] = int(episode_length)
+    # episode metrics (scenario_metrics, covid19_env.py:1613-1687): state names of the keys, the usa/ rates' divisor
+    p["state_names"] = [mc["US_STATE_IDX_TO_STATE_NAME"][str(a)] for a in range(S)]
+    p["us_population"] = int(us_pop)
     p["population"] = pop
     p["num_stringency_levels"] = int(mc["NUM_STRINGENCY_LEVELS"])
     assert int(n_stringency_levels) == p["num_stringency_levels"], \
@@ -223,7 +226,7 @@ class CovidBatchedEnv:
                  flatten_masks=True, collate_agent_step_and_reset_data=True, allow_observation_scaling=True,
                  use_real_world_data=False, use_real_world_policies=False, n_envs=1, device="cuda:0", auto_reset=True,
                  stepper_factory=None, seed=None, seeds=None, dense_log_frequency=None, world_dense_log_frequency=50,
-                 obs_dtype=None, final_obs=False, **scenario_kwargs):
+                 obs_dtype=None, final_obs=False, episode_metrics=False, **scenario_kwargs):
         from .._abi import obs_dtype_name
         self._obs_dtype = obs_dtype_name(obs_dtype)
         if final_obs and not auto_reset:
@@ -262,7 +265,8 @@ class CovidBatchedEnv:
         if stepper_factory is None:
             from ..covid_stepper import CudaCovidStepper
             self._stepper = CudaCovidStepper(self.params, self.n_envs, device=device, auto_reset=auto_reset,
-                                             final_obs=bool(final_obs), obs_dtype=self._obs_dtype)
+                                             final_obs=bool(final_obs), obs_dtype=self._obs_dtype,
+                                             episode_metrics=bool(episode_metrics))
         else:
             # a factory gets final_obs / obs_dtype only when they differ from the defaults, so a three-argument
             # factory keeps working for a default env
@@ -271,7 +275,12 @@ class CovidBatchedEnv:
                 kw["final_obs"] = True
             if self._obs_dtype != "float32":
                 kw["obs_dtype"] = self._obs_dtype
+            if episode_metrics:
+                kw["episode_metrics"] = True
             self._stepper = stepper_factory(self.params, self.n_envs, auto_reset, **kw)
+            if episode_metrics and not getattr(self._stepper, "episode_metrics_on", False):
+                raise NotImplementedError("episode_metrics=True: the stepper made by stepper_factory keeps no episode-metric "
+                                          "accumulators (it needs aie_covid_bind_metrics buffers)")
             if final_obs and not getattr(self._stepper, "final_obs", False):
                 raise NotImplementedError("final_obs=True: the stepper made by stepper_factory does not write final "
                                           "observations (it needs final_<name> buffers and a final-observation step)")
@@ -279,6 +288,7 @@ class CovidBatchedEnv:
                 raise NotImplementedError("obs_dtype=%s: the stepper made by stepper_factory writes %s observations"
                                           % (self._obs_dtype, getattr(self._stepper, "obs_dtype", "float32")))
         self._final_obs = bool(final_obs)
+        self._episode_metrics = bool(episode_metrics)
         self._loaded = False
         self._rollout = None   # bind_rollout
         self._build_views()
@@ -420,6 +430,65 @@ class CovidBatchedEnv:
         per_episode_end=True, the values of its [K, ...] final slots."""
         return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam,
                                                 per_episode_end=per_episode_end)
+
+    # ------------------------------------------------------------------ episode metrics (episode_metrics=True)
+    # scenario_metrics() (covid19_env.py:1613-1687) of every replica, from accumulators the step kernel keeps on the
+    # device: float64 time sums of the stored float32 series, float32 index sums as the reference keeps them.  A row is
+    # one launch away from metrics_tensor(); the dict forms copy it to the host.  Every replica ends its episodes on the
+    # same step, so previous_episode_metrics exists for all of them or for none.
+    def _need_metrics(self):
+        if not self._episode_metrics:
+            raise ValueError("episode metrics need make_env_instance(\"CovidAndEconomySimulation\", ..., "
+                             "episode_metrics=True)")
+        assert self._loaded, "call reset() first"
+
+    @property
+    def metric_keys(self):
+        """Column order of metrics_tensor() / previous_episode_metrics_tensor(): the reference's scenario_metrics() keys,
+        eight per state ("<state name>/<field>") then seven "usa/<field>", K = 8 * 51 + 7 = 415."""
+        self._need_metrics()
+        return [k for k, _ in self._stepper.metric_layout()]
+
+    def metrics_tensor(self, out=None):
+        """scenario_metrics() of every replica's running episode as one float64 tensor [n_envs, K] on the device (columns:
+        metric_keys), one kernel launch, no synchronisation.  Mid-episode the time means divide by episode_length, as the
+        reference's zero-padded global_state does.  out: an optional contiguous float64 [n_envs, K] tensor."""
+        self._need_metrics()
+        return self._stepper.episode_metrics(final=False, out=out)
+
+    def previous_episode_metrics_tensor(self, out=None):
+        """scenario_metrics() of the episode every replica finished last, float64 [n_envs, K] on the device, one launch.
+        Before any episode has ended the library's AieError is raised (previous_episode_metrics is None then)."""
+        self._need_metrics()
+        return self._stepper.episode_metrics(final=True, out=out)
+
+    def metrics_rows_as_dicts(self, rows, envs=None):
+        """Rows of metrics_tensor() / previous_episode_metrics_tensor() ([n, K], tensor or array) as the dicts
+        metrics_of(e) returns, in metric_keys order (floats).  envs: the row indices (default: all).  Copies to the host."""
+        self._need_metrics()
+        a = rows.detach().cpu().numpy() if hasattr(rows, "detach") else np.asarray(rows)
+        a = np.asarray(a, np.float64).reshape(-1, a.shape[-1])
+        keys = self.metric_keys
+        return [dict(zip(keys, a[int(e)].tolist())) for e in (range(a.shape[0]) if envs is None else envs)]
+
+    @property
+    def metrics(self):
+        """scenario_metrics() of replica 0's running episode (BaseEnvironment.metrics)."""
+        return self.metrics_of(0)
+
+    def metrics_of(self, e):
+        return self.metrics_rows_as_dicts(self.metrics_tensor(), envs=[e])[0]
+
+    @property
+    def previous_episode_metrics(self):
+        """scenario_metrics() of the episode replica 0 finished last; None before any has ended."""
+        return self.previous_episode_metrics_of(0)
+
+    def previous_episode_metrics_of(self, e):
+        self._need_metrics()
+        if not self._stepper.has_previous_episode():
+            return None
+        return self.metrics_rows_as_dicts(self.previous_episode_metrics_tensor(), envs=[e])[0]
 
     def _build_views(self):
         b = self._stepper.buf

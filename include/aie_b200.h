@@ -756,6 +756,42 @@ int aie_covid_rollout_restart(aie_covid_env *env, void *stream);
 /* aie_compute_advantages_k for the COVID-19 scenario, A = S states. */
 int aie_covid_compute_advantages_k(aie_covid_env *env, const aie_advantage_args *args, int32_t T, int32_t K, void *stream);
 
+/* ABI 6 (additive).  Episode metrics of the COVID-19 scenario: CovidAndEconomySimulation.scenario_metrics()
+ * (covid19_env.py:1613-1687) of every replica, from accumulators the step kernel keeps in caller-owned DEVICE buffers.
+ * Two blocks per replica, "current" (the running episode) and "previous" (the episode it finished last):
+ *   sums / prev_sums    float64 [E, 4, S]: sums over t = 1..t of the float32 Unemployed, Stringency Level,
+ *                       Postsubsidy Productivity and Subsidy the step stores, in step order
+ *   index / prev_index  float32 [E, 2, S + 1]: Health Index then Economic Index, of each state then the planner, each
+ *                       the float32 running sum of the step's marginal index (covid19_env.py:1124-1125, 1160-1161)
+ *   prev_end            float32 [E, 4, S]: I, R, D, V of the state the previous episode ended in
+ *   us_population       the divisor of the usa/ rates (model_constants.json US_POPULATION)
+ * While bound, every step kernel adds to the current block (the same launches as without, in kernel variants that also
+ * accumulate); the step that ends an episode under the auto-reset copies it, with the end state, to the previous block
+ * and zeroes it, before the reset.  aie_covid_reset zeroes the current block, and accumulation counts from there: bind,
+ * then reset.  m == NULL unbinds.  No launch.  AIE_EINVAL for a NULL pointer, a pointer not aligned to its element or
+ * us_population <= 0; AIE_ESTATE before aie_covid_bind_buffers or while a rollout is bound. */
+typedef struct aie_covid_metric_buffers {
+    double *sums, *prev_sums;
+    float *index, *prev_index, *prev_end;
+    double us_population;
+} aie_covid_metric_buffers;
+int aie_covid_bind_metrics(aie_covid_env *env, const aie_covid_metric_buffers *m);
+/* The columns of aie_covid_episode_metrics, in the reference's dict order: for each state s = 0..S-1 the eight fields
+ * "infected (millions)", "recovered (millions)", "deaths (millions)", "mean_unemployment_rate (%)",
+ * "mean_open_close_stringency_level", "total_productivity (billion $)", "health_index_at_end_of_episode",
+ * "economic_index_at_end_of_episode" (state = s; the key is "<state name>/<field>"), then seven with state = -1 (key
+ * "usa/<field>").  The library holds no state names.  Fills at most cap entries, returns K = 8 S + 7 (or a negative
+ * AIE_E* code). */
+typedef struct aie_covid_metric_column { int32_t state; char field[60]; } aie_covid_metric_column;
+int aie_covid_get_metric_layout(const aie_covid_env *env, aie_covid_metric_column *out, int32_t cap);
+/* One launch (aie_covid_metrics_kernel: one CTA per replica, one thread per state) writes float64 [n_envs, K] to the
+ * DEVICE buffer out.  source 0: the current block and the live state (env.metrics mid-episode: the time means divide by
+ * episode_length, as the reference's zero-padded global_state does); 1: the previous block (previous_episode_metrics).
+ * Each value is float64 arithmetic in a fixed order (USA sums over the states in index order).  Asynchronous on
+ * `stream`.  AIE_EINVAL for a NULL or misaligned out or an unknown source; AIE_ESTATE without bound metric buffers,
+ * before aie_covid_reset has run since they were bound, or for source 1 before an episode has ended since then. */
+int aie_covid_episode_metrics(aie_covid_env *env, int32_t source, double *out, void *stream);
+
 const char *aie_last_error(void);
 int aie_abi_version(void);
 
