@@ -150,9 +150,13 @@ static void emu_auto_reset(aie_env *env, int e, uint8_t *img, uint8_t *grec) {
                   episodes = hdr[HDR_EPISODES] + 1, saez_n = hdr[HDR_SAEZ_N];
     const uint8_t *snap = b.state0 + (size_t)e * c.rec_bytes;
     const size_t tail = (size_t)(c.rec_bytes - c.off_price_hist);
-    if (b.final) {   // the resident record as it stands; a split record's statistics come from global memory
+    if (b.final) {   // the resident record as it stands; a split record's statistics and price history (which the final
+                     // observation pass reads) come from global memory
         memcpy(b.final + (size_t)e * c.rec_bytes, img, c.resident_bytes);
-        if (c.split) memcpy(b.final + (size_t)e * c.rec_bytes + c.off_stats, grec + c.off_stats, 16 * ((8 * (size_t)c.n_stats + 15) / 16));
+        if (c.split) {
+            memcpy(b.final + (size_t)e * c.rec_bytes + c.off_stats, grec + c.off_stats, 16 * ((8 * (size_t)c.n_stats + 15) / 16));
+            memcpy(b.final + (size_t)e * c.rec_bytes + c.off_price_hist, grec + c.off_price_hist, 16 * ((size_t)(c.off_orders - c.off_price_hist) / 16));
+        }
     }
     memcpy(img, snap, c.off_mt);
     memcpy((c.split ? grec : img) + c.off_price_hist, snap + c.off_price_hist, tail);

@@ -84,9 +84,11 @@ def _random_steps(dev, host, n, rng):
         host.step((acts, pa) if pa is not None else acts)
 
 
-def _twin(cfg, factory, E=5, seeds=None, rounds=None, auto_reset=False, **over):
+def _twin(cfg, factory, E=5, seeds=None, rounds=None, auto_reset=False, compare=None, **over):
     """First reset, then further explicit resets after random steps: rounds lists the steps before each of them (the
-    default ends one episode exactly, waiting for its reset, and leaves the next unfinished)."""
+    default ends one episode exactly, waiting for its reset, and leaves the next unfinished).  compare(dev, host, label)
+    checks every reset (default: _compare, byte-identical)."""
+    compare = compare or _compare
     dev = _make(cfg, E, factory, auto_reset=auto_reset, **over)
     host = _make(cfg, E, factory, auto_reset=auto_reset, **over)
     assert dev.spec["reset_mode"] == 1
@@ -95,14 +97,14 @@ def _twin(cfg, factory, E=5, seeds=None, rounds=None, auto_reset=False, **over):
     host.seed(seeds)
     dev.reset()
     _host_reset(host)
-    _compare(dev, host, "first reset")
+    compare(dev, host, "first reset")
     T = dev.episode_length
     rng = np.random.RandomState(sum(seeds))
     for r, n in enumerate(rounds if rounds is not None else [T, min(3, T - 1)]):
         _random_steps(dev, host, n, rng)
         dev.reset()
         _host_reset(host)
-        _compare(dev, host, "reset %d after %d steps" % (r + 2, n))
+        compare(dev, host, "reset %d after %d steps" % (r + 2, n))
     return dev, host
 
 
@@ -270,8 +272,10 @@ def test_emulated_reset_envs_abi_errors():
 SKILL_FIELDS = ("build_payment", "build_skill", "bonus_gather_prob", "gauss_state")
 
 
-def _compare_large(dev, other, label, libm_fields=SKILL_FIELDS):
-    """Record / output bytes of every replica (the streams are inside the records); stream_state of a few replicas."""
+def _compare_large(dev, other, label, libm_fields=SKILL_FIELDS, libm_bufs=()):
+    """Record / output bytes of every replica (the streams are inside the records); stream_state of a few replicas.
+    libm_bufs: float64 output buffers computed with exp / log / pow (the rewards after a step: differences of two
+    utilities, so an ulp of a utility is an absolute error), held to 1e-12 relative or absolute."""
     sd, so = dev.stepper, other.stepper
     skill = []
     for f in libm_fields:
@@ -289,6 +293,10 @@ def _compare_large(dev, other, label, libm_fields=SKILL_FIELDS):
                 x, y = a[:, lo:hi].copy().view(np.float64), b[:, lo:hi].copy().view(np.float64)
                 assert np.allclose(x, y, rtol=1e-12, atol=0), "%s: %s skills" % (label, k)
                 a[:, lo:hi] = b[:, lo:hi]
+        elif k in libm_bufs:
+            assert np.allclose(a, b, rtol=1e-12, atol=1e-12), "%s: %s (max abs difference %g)" % (
+                label, k, np.abs(a - b).max())
+            continue
         elif a.dtype == np.float32 and not np.array_equal(a, b):
             assert np.allclose(a, b, rtol=1e-6, atol=0), "%s: %s" % (label, k)
             continue
