@@ -198,6 +198,18 @@ class AieCovidMetricColumn(C.Structure):
     _fields_ = [("state", C.c_int32), ("field", C.c_char * 60)]
 
 
+class AieCounters(C.Structure):
+    """aie_counters: the host-side counters of a handle (aie_get_counters / aie_set_counters)."""
+    _fields_ = [("sample_calls", C.c_uint64), ("policy_calls", C.c_uint64), ("fused_policy_key", C.c_uint64),
+                ("fused_policy_on", C.c_int32), ("reserved", C.c_int32)]
+
+
+class AieCovidCounters(C.Structure):
+    """aie_covid_counters: the host-side counters of a COVID-19 handle (aie_covid_get_counters / _set_counters)."""
+    _fields_ = [("sample_calls", C.c_uint64), ("policy_calls", C.c_uint64), ("t", C.c_int32),
+                ("previous_episode", C.c_int32)]
+
+
 class AieCovidRollout(C.Structure):
     """aie_covid_rollout: the device tensors of a COVID-19 rollout stored in place (aie_covid_bind_rollout)."""
     _fields_ = [("T", C.c_int32), ("obs", AieCovidObsBuffers), ("actions_agent", C.c_void_p),
@@ -298,6 +310,10 @@ def load_library(path=None):
                "aie_step", "aie_observe", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_read_state", "aie_step_dynamics",
                "aie_sample_random_actions", "aie_set_fused_policy"]:
         getattr(L, fn).restype = C.c_int
+    for fn, st in (("aie_get_counters", AieCounters), ("aie_set_counters", AieCounters),
+                   ("aie_covid_get_counters", AieCovidCounters), ("aie_covid_set_counters", AieCovidCounters)):
+        getattr(L, fn).argtypes = [P, C.POINTER(st)]
+        getattr(L, fn).restype = C.c_int
     if L.aie_abi_version() != ABI_VERSION:
         raise AieError("ABI version mismatch between %s and the Python binding" % path)
     return L
@@ -307,6 +323,7 @@ EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field"
                     "aie_load_state", "aie_reset_envs", "aie_step", "aie_step_dynamics", "aie_observe", "aie_observe_final", "aie_sample_random_actions",
                     "aie_set_fused_policy", "aie_sample_policy", "aie_evaluate_policy", "aie_evaluate_policy_backward", "aie_compute_advantages", "aie_compute_advantages_k", "aie_bind_rollout", "aie_rollout_restart", "aie_step_host", "aie_step_host_compact", "aie_compact_bytes_per_env", "aie_get_host_timing", "aie_read_state", "aie_read_episode_final",
                     "aie_get_metric_layout", "aie_episode_metrics", "aie_launch_count", "aie_last_error", "aie_abi_version",
+                    "aie_get_counters", "aie_set_counters", "aie_covid_get_counters", "aie_covid_set_counters",
                     "aie_covid_create", "aie_covid_destroy", "aie_covid_bind_buffers", "aie_covid_reset", "aie_covid_step",
                     "aie_covid_step_final", "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
                     "aie_covid_evaluate_policy_backward", "aie_covid_compute_advantages", "aie_covid_launch_count",

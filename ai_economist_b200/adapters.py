@@ -196,6 +196,27 @@ class MultiAgentDictEnv:
         self.env.reset()
         return self.env.reference_view(self.e)[0]
 
+    # ---- checkpoints (tutorials/rllib/env_wrapper.py:155-165, pickle_file): the whole batched env, every replica ----
+    pickle_file = "game_object.pt"
+
+    def save_game_object(self, save_dir):
+        """Write env.state_dict() to save_dir/game_object.pt (torch.save)."""
+        import os
+
+        import torch
+        assert os.path.isdir(save_dir)
+        torch.save(self.env.state_dict(), os.path.join(save_dir, self.pickle_file))
+
+    def load_game_object(self, save_dir):
+        """Load save_dir/game_object.pt into the wrapped env (load_state_dict), which must have the configuration of the
+        env it was saved from."""
+        import os
+
+        import torch
+        assert os.path.isdir(save_dir)
+        # the dict holds numpy arrays and plain Python values next to tensors: not a weights-only file
+        self.env.load_state_dict(torch.load(os.path.join(save_dir, self.pickle_file), weights_only=False))
+
     def step(self, action_dict):
         """action_dict: {agent id: int | list} for this replica; the other replicas take NO-OPs."""
         st = self.env.stepper

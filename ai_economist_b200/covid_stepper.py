@@ -248,6 +248,21 @@ class CovidStepperBase(PolicySampler):
     def launch_count(self):
         return int(self.lib.aie_covid_launch_count(self._h))
 
+    def get_counters(self):
+        """The library's host-side counters of this handle (aie_covid_get_counters) and this driver's mirror of the
+        lock-step timestep, as a dict of ints."""
+        c = _abi.AieCovidCounters()
+        self._check(self.lib.aie_covid_get_counters(self._h, C.byref(c)))
+        out = {k: int(getattr(c, k)) for k, _ in _abi.AieCovidCounters._fields_}
+        out.update(host_t=int(self._t), host_ended=int(self._ended))
+        return out
+
+    def set_counters(self, counters):
+        """Write the counters of get_counters() back (aie_covid_set_counters); marks the buffers as reset."""
+        c = _abi.AieCovidCounters(**{k: int(counters[k]) for k, _ in _abi.AieCovidCounters._fields_})
+        self._check(self.lib.aie_covid_set_counters(self._h, C.byref(c)))
+        self._t, self._ended = int(counters["host_t"]), bool(counters["host_ended"])
+
     # -- episode metrics (aie_covid_bind_metrics / aie_covid_episode_metrics) -------------------------------------------
     def metric_layout(self):
         """[(key, is_int)] of the metric columns: "<state name>/<field>" for each state, then "usa/<field>" (the

@@ -693,6 +693,118 @@ class BatchedFoundationEnv:
         return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam,
                                                 per_episode_end=per_episode_end)
 
+    # ------------------------------------------------------------------ checkpoints
+    def _checkpoint_config(self):
+        """What a checkpoint must have been taken from to load into this env (load_state_dict checks each field)."""
+        from .._abi import ABI_VERSION
+        return dict(scenario=self.name, n_envs=self.n_envs, obs_dtype=self._spec["obs_dtype"], auto_reset=self._auto_reset,
+                    final_obs=self._spec["final_obs"],
+                    dense_log=[self._create_dense_log_every, self._world_dense_log_frequency], abi_version=ABI_VERSION,
+                    spec=self._spec)
+
+    def _checkpoint_buffers(self):
+        """name -> the buffer a checkpoint holds: the records, the event log, and the action / reward / done tensors
+        env.action_buffers / env.rew / env.done show (slot 0 of a bound rollout)."""
+        st = self._stepper
+        out = {k: st.buf[k] for k in ("state", "state0", "episode_final", "events") if k in st.buf}
+        out["actions_agent"], out["actions_planner"] = self.action_buffers
+        if self._rollout is None:
+            out["reward"], out["done"] = st.buf["reward"], st.buf["done"]
+        else:
+            out["reward"], out["done"] = self._rollout.buf["reward"][0], self._rollout.buf["done"][0]
+        if self._saez is not None:
+            # the host writes a new tax period's rates into the records after the step that observed the old ones, so the
+            # stand-alone pass would show the agents' marginal rates under the new rates: keep the step's observations
+            out.update(self.obs_tensors)
+        return out
+
+    def state_dict(self):
+        """The whole state of the batched env between steps, for resuming a run bit for bit: a dict of tensors (copies
+        on the env's device), numpy arrays and plain Python values that torch.save can write.  It holds every replica's
+        state record, its auto-reset snapshot and end-of-episode record, the action / reward / done buffers, the
+        library's sampler counters and fused-policy key, the completion counts, the Saez estimator, the dense log being
+        recorded and the host-side tables drawn at construction.  Observations are not stored (except under the Saez
+        tax model): load_state_dict() re-derives them from the records.  Allowed after the first reset(); with a rollout
+        bound only at slot 0 (ValueError otherwise)."""
+        from . import checkpoint as ck
+        if not self._loaded:
+            raise ValueError("state_dict: nothing to save before the first reset()")
+        ck.refuse_mid_rollout(self, "state_dict")
+        if not hasattr(self._stepper, "get_counters"):
+            raise NotImplementedError("this env's stepper keeps no checkpointable counters")
+        buffers = {k: ck.snapshot(v) for k, v in self._checkpoint_buffers().items()}
+        rs = self._rs if self._rs is not None else []
+        host = dict(completions=self._completions.copy(), last_ep_metrics=getattr(self, "_last_ep_metrics_host", None),
+                    gauss_has=np.array([s.get_state()[3] for s in rs], np.int64),
+                    gauss_val=np.array([s.get_state()[4] for s in rs], np.float64),
+                    dense_log=self._dense_log, last_ep_dense_log=self._last_ep_dense_log, dense_logger=None,
+                    saez=self._saez.state_dict() if self._saez is not None else None)
+        lg = self._dense_logger
+        if lg is not None:
+            host["dense_logger"] = dict(log=lg.log, comp=lg.comp, paid_prev=lg._paid_prev, static=lg._static)
+        # host tables drawn from the seeded streams at construction (a resumed env is made with other seeds)
+        if hasattr(self.scenario, "_split_ranked_skill"):
+            host["split_ranked_skill"] = self.scenario._split_ranked_skill
+        labor = self._components_dict.get("SimpleLabor")
+        if labor is not None:
+            host["labor_skills"] = labor.skills
+        return dict(format_version=ck.FORMAT_VERSION, config=ck.plain(self._checkpoint_config()), buffers=buffers,
+                    counters=self._stepper.get_counters(), host=ck.host_copy(host))
+
+    def load_state_dict(self, sd):
+        """Load a state_dict() taken from an env of the same configuration (scenario, numeric spec, n_envs, obs_dtype,
+        auto_reset, final_obs, dense-log settings, ABI and format version: ValueError naming the field otherwise) into
+        this env's own buffers, then re-derive the observations (and, with final_obs and no rollout bound, the final
+        observations of the replicas whose done flag is set) with the stand-alone observation pass.  Returns env.obs.
+        From here on every call returns what
+        it would have returned in the env the dict was taken from.  Allowed on a new env before any reset(), and between
+        steps; with a rollout bound only at slot 0 (the observations go into slot 0)."""
+        from . import checkpoint as ck
+        ck.check_config(sd, self._checkpoint_config())
+        ck.refuse_mid_rollout(self, "load_state_dict")
+        st = self._stepper
+        mine = self._checkpoint_buffers()
+        if set(sd["buffers"]) != set(mine):
+            raise ValueError("load_state_dict: the checkpoint holds buffers %s, this env %s"
+                             % (sorted(sd["buffers"]), sorted(mine)))
+        for k, dst in mine.items():
+            ck.copy_into(dst, sd["buffers"][k], k)
+        host = ck.host_copy(sd["host"])
+        counters = dict(sd["counters"])
+        # the stand-alone pass would draw the fused random policy's next actions over the restored ones: run it with the
+        # policy off, then restore the key
+        st.set_counters(dict(counters, fused_policy_key=0, fused_policy_on=0))
+        if self._saez is None:
+            st.observe()
+        if self._rollout is None and getattr(st, "final_obs", False):
+            st.observe_final()
+        st.set_counters(counters)
+        self._loaded = True
+        self._completions = np.asarray(host["completions"], np.int64).copy()
+        if host["last_ep_metrics"] is not None:
+            self._last_ep_metrics_host = host["last_ep_metrics"]
+        elif hasattr(self, "_last_ep_metrics_host"):
+            del self._last_ep_metrics_host
+        if self._rs is None:
+            self._rs = [np.random.RandomState() for _ in range(self.n_envs)]
+        for rs, has, val in zip(self._rs, host["gauss_has"], host["gauss_val"]):
+            s = rs.get_state()   # the key and position are the record's (synchronised before every host use)
+            rs.set_state((s[0], s[1], s[2], int(has), float(val)))
+        if "split_ranked_skill" in host:
+            self.scenario._split_ranked_skill = np.asarray(host["split_ranked_skill"], np.float64)
+        if "labor_skills" in host:
+            self._components_dict["SimpleLabor"].skills = np.asarray(host["labor_skills"])
+        if self._saez is not None:
+            self._saez.load_state_dict(host["saez"])
+        self._dense_log, self._last_ep_dense_log = host["dense_log"], host["last_ep_dense_log"]
+        self._dense_logger = None
+        if host["dense_logger"] is not None:
+            from .dense_log import DenseLogger
+            lg = self._dense_logger = DenseLogger(self, 0, self._world_dense_log_frequency)
+            d = host["dense_logger"]
+            lg.log, lg.comp, lg._paid_prev, lg._static = d["log"], d["comp"], d["paid_prev"], d["static"]
+        return self.obs
+
     # ------------------------------------------------------------------ outputs
     @staticmethod
     def _named_fields(flat, layout):

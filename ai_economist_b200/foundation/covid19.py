@@ -15,6 +15,8 @@ from datetime import datetime
 
 import numpy as np
 
+from .._abi import COVID_OBS_NAMES
+
 DATA_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "covid19_data")
 F32, I32 = np.float32, np.int32
 
@@ -607,6 +609,64 @@ class CovidBatchedEnv:
                 import torch
                 self._final_rate_p.copy_(torch.where(done, last, self._final_rate_p))
                 self._final_rate_a.copy_(torch.where(done[:, None], last, self._final_rate_a))
+
+    # ------------------------------------------------------------------ checkpoints
+    def _checkpoint_config(self):
+        from .._abi import ABI_VERSION
+        return dict(scenario=self.name, n_envs=self.n_envs, obs_dtype=self._obs_dtype,
+                    auto_reset=getattr(self._stepper, "_auto_reset", None), final_obs=self._final_obs,
+                    episode_metrics=self._episode_metrics, observe_rate=self._rate_tab is not None,
+                    abi_version=ABI_VERSION, spec=self.params)
+
+    def _checkpoint_buffers(self):
+        """name -> the buffer a checkpoint holds: the simulation state, the observations, masks, rewards, done and
+        actions env.obs / env.rew / env.done / env.action_buffers show (slot 0 of a bound rollout), the final
+        observations, the rate observations and the episode-metric accumulators."""
+        st, r = self._stepper, self._rollout
+        out = {k: st.buf[k] for k in ("state", "ints", "hdr", "ring", "changes") if k in st.buf}
+        obs = st.buf if r is None else r.obs_slots[0]
+        out.update({k: obs[k] for k in COVID_OBS_NAMES})
+        out["actions_agent"], out["actions_planner"] = self.action_buffers
+        src = st.buf if r is None else {k: r.buf[k][0] for k in ("reward_agent", "reward_planner", "done")}
+        out.update({k: src[k] for k in ("reward_agent", "reward_planner", "done")})
+        out.update({k: v for k, v in st.buf.items() if k.startswith("final_") or k.startswith("metric_")})
+        if self._rate_tab is not None:
+            out["rate_agent"], out["rate_planner"] = self._rate_a, self._rate_p
+            if self._final_obs:
+                out["final_rate_agent"], out["final_rate_planner"] = self._final_rate_a, self._final_rate_p
+        return out
+
+    def state_dict(self):
+        """The whole state of the batched env between steps (the contract of BatchedFoundationEnv.state_dict): the
+        simulation buffers, observations, rewards, actions, final observations and metric accumulators (copies on the
+        env's device), the library's sampler counters and the lock-step timestep.  Allowed after the first reset();
+        with a rollout bound only at slot 0 (ValueError otherwise)."""
+        from . import checkpoint as ck
+        if not self._loaded:
+            raise ValueError("state_dict: nothing to save before the first reset()")
+        ck.refuse_mid_rollout(self, "state_dict")
+        if not hasattr(self._stepper, "get_counters"):
+            raise NotImplementedError("this env's stepper keeps no checkpointable counters")
+        return dict(format_version=ck.FORMAT_VERSION, config=ck.plain(self._checkpoint_config()),
+                    buffers={k: ck.snapshot(v) for k, v in self._checkpoint_buffers().items()},
+                    counters=self._stepper.get_counters())
+
+    def load_state_dict(self, sd):
+        """Load a state_dict() taken from an env of the same configuration (ValueError naming the field that differs)
+        into this env's own buffers; with a rollout bound only at slot 0, whose observations it writes.  Allowed on a
+        new env before any reset()."""
+        from . import checkpoint as ck
+        ck.check_config(sd, self._checkpoint_config())
+        ck.refuse_mid_rollout(self, "load_state_dict")
+        mine = self._checkpoint_buffers()
+        if set(sd["buffers"]) != set(mine):
+            raise ValueError("load_state_dict: the checkpoint holds buffers %s, this env %s"
+                             % (sorted(sd["buffers"]), sorted(mine)))
+        for k, dst in mine.items():
+            ck.copy_into(dst, sd["buffers"][k], k)
+        self._stepper.set_counters(sd["counters"])
+        self._loaded = True
+        return self.obs
 
     def reset(self):
         self._stepper.reset()

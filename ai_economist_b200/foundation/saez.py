@@ -336,6 +336,42 @@ class SaezHost:
         self._seen = np.zeros(env.n_envs, np.int64)   # samples already copied from the device, per replica
         self.elas_at_episode_end = [None] * env.n_envs  # saez/estimated_elasticity of previous_episode_metrics
 
+    _SMOOTHED = ("elas_tm1", "elas_t", "log_z0_tm1", "log_z0_t")
+
+    def state_dict(self):
+        """The estimator's whole state (numpy arrays and Python values; BatchedFoundationEnv.state_dict)."""
+        b = self.batch
+        if isinstance(b, SaezLoop):
+            out = dict(kind="loop", buffers=[np.array(e.buffer, np.float64).reshape(-1, 2) for e in b.est],
+                       running_avg=np.stack([e.running_avg for e in b.est]).copy())
+            out.update({k: np.array([getattr(e, k) for e in b.est], np.float64) for k in self._SMOOTHED})
+        else:
+            out = dict(kind="batch", buf=b.buf.copy(), count=b.count.copy(), start=b.start.copy(),
+                       running_avg=b.running_avg.copy())
+            out.update({k: getattr(b, k).copy() for k in self._SMOOTHED})
+        out.update(seen=self._seen.copy(), elas_at_episode_end=list(self.elas_at_episode_end))
+        return out
+
+    def load_state_dict(self, sd):
+        b = self.batch
+        kind = "loop" if isinstance(b, SaezLoop) else "batch"
+        if sd.get("kind") != kind:
+            raise ValueError("load_state_dict: the Saez estimator of the checkpoint is %r, this env's is %r"
+                             % (sd.get("kind"), kind))
+        if kind == "loop":
+            for e, est in enumerate(b.est):
+                est.buffer = [[float(z), float(tau)] for z, tau in np.asarray(sd["buffers"][e], np.float64)]
+                est.running_avg = np.array(sd["running_avg"][e], np.float64)
+                for k in self._SMOOTHED:
+                    setattr(est, k, float(sd[k][e]))
+        else:
+            b.buf[...], b.count[...], b.start[...] = sd["buf"], sd["count"], sd["start"]
+            b.running_avg[...] = sd["running_avg"]
+            for k in self._SMOOTHED:
+                getattr(b, k)[...] = sd[k]
+        self._seen[...] = sd["seen"]
+        self.elas_at_episode_end = [None if v is None else float(v) for v in sd["elas_at_episode_end"]]
+
     def _np(self, name, final=False):
         st = self.env.stepper
         return st.to_numpy(st.state_view(name, final=final))

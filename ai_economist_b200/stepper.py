@@ -727,6 +727,17 @@ class BatchStepper(PolicySampler):
     def launch_count(self):
         return int(self.lib.aie_launch_count(self._h))
 
+    def get_counters(self):
+        """The library's host-side counters of this handle (aie_get_counters) as a dict of ints."""
+        c = _abi.AieCounters()
+        self._check(self.lib.aie_get_counters(self._h, C.byref(c)))
+        return {k: int(getattr(c, k)) for k, _ in _abi.AieCounters._fields_ if k != "reserved"}
+
+    def set_counters(self, counters):
+        """Write the counters of get_counters() back (aie_set_counters); marks the records as loaded."""
+        c = _abi.AieCounters(**{k: int(v) for k, v in counters.items()})
+        self._check(self.lib.aie_set_counters(self._h, C.byref(c)))
+
     def field(self, name):
         if name not in self._fields:
             f = _abi.AieField()

@@ -609,6 +609,24 @@ int aie_episode_metrics(aie_env *env, int32_t source, double *out, void *stream)
 /* Number of kernels the library has launched on this handle since creation (for bench "gpu_launches"). */
 int64_t aie_launch_count(const aie_env *env);
 
+/* ABI 6 (additive).  The counters the library keeps on the host for a handle, beyond what the caller's buffers hold:
+ * with them and every record of state / state0 / episode_final, a checkpoint of an env resumes bit for bit. */
+typedef struct aie_counters {
+    uint64_t sample_calls;       /* aie_sample_random_actions calls, aie_set_fused_policy's own draw included */
+    uint64_t policy_calls;       /* aie_sample_policy calls (the policy sampler's stream counter n) */
+    uint64_t fused_policy_key;   /* the fused random policy's key, host_mix64(seed) | 1; 0 when it is off */
+    int32_t fused_policy_on;     /* 1: the fused random policy is on (fused_policy_key != 0), 0: off */
+    int32_t reserved;            /* 0 */
+} aie_counters;
+/* Reads the counters into *out.  aie_set_counters writes them back and marks the env loaded: the caller has written
+ * every record of state and state0 (and episode_final) itself, from an env of the same configuration, so aie_step and
+ * aie_observe may follow without aie_load_state.  Neither call launches anything; the launch count is diagnostic and
+ * is neither read nor written.  AIE_EINVAL for a NULL env or counters, and (set) fused_policy_on not 0 or 1, or not
+ * matching fused_policy_key != 0; AIE_ESTATE before aie_bind_buffers, while a rollout is bound at s != 0, and (set) a
+ * fused policy that is on while a rollout is bound. */
+int aie_get_counters(aie_env *env, aie_counters *out);
+int aie_set_counters(aie_env *env, const aie_counters *in);
+
 /* ================================================================================================
  * COVID-19 + economy scenario (BASELINE config 4)
  *
@@ -791,6 +809,20 @@ int aie_covid_get_metric_layout(const aie_covid_env *env, aie_covid_metric_colum
  * `stream`.  AIE_EINVAL for a NULL or misaligned out or an unknown source; AIE_ESTATE without bound metric buffers,
  * before aie_covid_reset has run since they were bound, or for source 1 before an episode has ended since then. */
 int aie_covid_episode_metrics(aie_covid_env *env, int32_t source, double *out, void *stream);
+
+/* ABI 6 (additive).  The host-side counters of a COVID-19 handle (the contract of aie_get_counters / aie_set_counters):
+ * with them and the caller's buffers (state, ints, hdr, ring, changes, and the metric accumulators when bound) a
+ * checkpoint resumes bit for bit.  aie_covid_set_counters marks the env reset (the caller has written its buffers),
+ * with its metric accumulators live when they are bound.  AIE_EINVAL for a NULL env or counters, and (set) t < 0 or
+ * previous_episode not 0 or 1; AIE_ESTATE before aie_covid_bind_buffers or while a rollout is bound at s != 0. */
+typedef struct aie_covid_counters {
+    uint64_t sample_calls;       /* aie_covid_sample_random_actions calls */
+    uint64_t policy_calls;       /* aie_covid_sample_policy calls */
+    int32_t t;                   /* the replicas' lock-step timestep */
+    int32_t previous_episode;    /* 1: an episode has ended since the metric buffers were bound (source 1 is valid) */
+} aie_covid_counters;
+int aie_covid_get_counters(aie_covid_env *env, aie_covid_counters *out);
+int aie_covid_set_counters(aie_covid_env *env, const aie_covid_counters *in);
 
 const char *aie_last_error(void);
 int aie_abi_version(void);
