@@ -7,6 +7,7 @@ import os
 ABI_VERSION = 6
 MAX_COMPONENTS, MAX_BRACKETS, MAX_RATES = 8, 16, 64
 AIE_OK = 0
+AIE_ESTATE = -3   # a call out of order (include/aie_b200.h)
 OBS_F32, OBS_BF16 = 0, 1   # aie_config.obs_dtype, aie_covid_config.obs_dtype
 REWARD_F32, REWARD_F64 = 0, 1   # aie_advantage_args.rewards_*_dtype
 
@@ -314,6 +315,11 @@ def load_library(path=None):
                    ("aie_covid_get_counters", AieCovidCounters), ("aie_covid_set_counters", AieCovidCounters)):
         getattr(L, fn).argtypes = [P, C.POINTER(st)]
         getattr(L, fn).restype = C.c_int
+    for fam in ("aie", "aie_covid"):   # captured rollouts
+        for fn, args in (("rollout_capture_begin", [P, P]), ("rollout_capture_end", [P]),
+                         ("rollout_replay_begin", [P, P]), ("rollout_replay_end", [P])):
+            getattr(L, "%s_%s" % (fam, fn)).argtypes = args
+            getattr(L, "%s_%s" % (fam, fn)).restype = C.c_int
     if L.aie_abi_version() != ABI_VERSION:
         raise AieError("ABI version mismatch between %s and the Python binding" % path)
     return L
@@ -328,7 +334,10 @@ EXPORTED_SYMBOLS = ["aie_create", "aie_destroy", "aie_get_dims", "aie_get_field"
                     "aie_covid_step_final", "aie_covid_sample_random_actions", "aie_covid_sample_policy", "aie_covid_evaluate_policy",
                     "aie_covid_evaluate_policy_backward", "aie_covid_compute_advantages", "aie_covid_launch_count",
                     "aie_covid_bind_rollout", "aie_covid_rollout_restart", "aie_covid_compute_advantages_k",
-                    "aie_covid_bind_metrics", "aie_covid_get_metric_layout", "aie_covid_episode_metrics"]
+                    "aie_covid_bind_metrics", "aie_covid_get_metric_layout", "aie_covid_episode_metrics",
+                    "aie_rollout_capture_begin", "aie_rollout_capture_end", "aie_rollout_replay_begin", "aie_rollout_replay_end",
+                    "aie_covid_rollout_capture_begin", "aie_covid_rollout_capture_end", "aie_covid_rollout_replay_begin",
+                    "aie_covid_rollout_replay_end"]
 
 
 def obs_dtype_name(obs_dtype):

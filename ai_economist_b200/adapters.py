@@ -262,6 +262,10 @@ class ReferenceApiEnv:
         raise NotImplementedError("the reference API steps one replica through host copies; bind rollouts on the "
                                   "batched env (reference_api=False)")
 
+    def capture_rollout(self, act):
+        raise ValueError("the reference API steps one replica through host copies; capture rollouts on the batched env "
+                         "(reference_api=False)")
+
     @property
     def _completions(self):                # int, like the reference's (tutorials/rllib/env_wrapper.py:176 reads it)
         return int(self._env.completions()[self._e])

@@ -142,7 +142,25 @@ class CovidStepperBase(PolicySampler):
 
     def _check(self, rc):
         if rc != _abi.AIE_OK:
+            self._refused_in_capture(rc)
             raise _abi.AieError("aie error %d: %s" % (rc, self.lib.aie_last_error().decode()))
+
+    # captured rollouts (PolicySampler.rollout_capture_begin ...): this driver's mirror of the lock-step timestep is put
+    # back at the end of a capture and advanced by T steps after a replay, as the library's own
+    _capture_prefix = "aie_covid"
+
+    def rollout_capture_begin(self):
+        super().rollout_capture_begin()
+        self._capture_host = (self._t, self._ended)
+
+    def rollout_capture_end(self):
+        super().rollout_capture_end()
+        self._t, self._ended = self._capture_host
+
+    def rollout_replay_end(self):
+        super().rollout_replay_end()
+        for _ in range(self.rollout.T):
+            self._stepped()
 
     def _stream(self):
         return None
@@ -312,6 +330,8 @@ class CovidStepperBase(PolicySampler):
 
 
 class CudaCovidStepper(CovidStepperBase):
+    supports_rollout_capture = True
+
     def __init__(self, params, n_envs, device="cuda:0", auto_reset=True, lib_path=None, change_list=None, final_obs=False,
                  obs_dtype=None, episode_metrics=False):
         import torch

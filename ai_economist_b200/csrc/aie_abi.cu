@@ -39,6 +39,11 @@
 //                          row (k, e), k = the env's earlier done flags in the rollout (aie_bind_rollout).
 //   aie_compute_advantages_k_kernel  aie_compute_advantages_kernel with final values [K][n] indexed by episode-end
 //                          ordinal (aie_compute_advantages_k).
+//   aie_sample_policy_counter_kernel, aie_covid_sample_policy_counter_kernel  the policy samplers of a captured rollout
+//                          (aie_rollout_capture_begin): their call key read from the handle's device counter.
+//   aie_covid_step_slot_kernel  the COVID-19 step of a captured rollout with final slots: the final row found on the
+//                          device from the rollout's done flags.
+//   aie_set_counter_kernel  one thread: the policy-sampler call count into the device counter (aie_rollout_replay_begin).
 // The step, observe and sampler kernels have *_bf16 twins (same bodies, bfloat16 observations and masks,
 // aie_config::obs_dtype == AIE_OBS_BF16); the launchers pick one from the config, with the same launch shape.
 #include <cuda_runtime.h>
@@ -132,6 +137,15 @@ int covid_launch_policy_eval(aie_covid_env *, const PolicyEvalBufs &p, int mt_bf
 int launch_advantages(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, void *stream);
 int launch_advantages_k(const AdvantageBufs &b, long long E, int ra64, int rp64, int T, int K, void *stream);
 int launch_observe_final_slots(aie_env *, const DevBufs &fb, const int32_t *done0, int s, int K, void *stream);
+// captured rollouts (aie_rollout_capture_begin); CUDA backend only - a host build of the device source runs the same
+// bodies serially in the entry points
+int launch_policy_counter(aie_env *, const PolicyBufs &p, int lt_bf16, uint64_t seed_mix, const uint64_t *base, uint64_t ord,
+                          void *stream);
+int covid_launch_policy_counter(aie_covid_env *, const PolicyBufs &p, int lt_bf16, uint64_t seed_mix, const uint64_t *base,
+                                uint64_t ord, void *stream);
+int covid_launch_step_slot(aie_covid_env *, const CovidBufs &fin, const int32_t *done0, int s, int K, void *stream);
+int launch_set_counter(uint64_t *dst, uint64_t v, void *stream);
+bool stream_capturing(void *stream);
 }  // namespace be
 }  // namespace aie
 
@@ -619,6 +633,19 @@ __global__ void __launch_bounds__(256, 2) aie_sample_policy_bf16_kernel(const __
                                                                      const PolicyBufs p, uint64_t seed, int per_unit) {
     policy_kernel_body<EXT, bf16_t, LT>(c, b, p, seed, per_unit);
 }
+// The policy sampler of a captured rollout (aie_rollout_capture_begin): the body above with its key read on the device
+// (policy_call_key), so that every replay draws from the call count current at aie_rollout_replay_begin.  MT: the
+// masks' element type, LT: the logits'.
+template <bool EXT, typename MT, typename LT>
+__global__ void __launch_bounds__(256, 2) aie_sample_policy_counter_kernel(const __grid_constant__ DevCfg c, const DevBufs b,
+                                                                        const PolicyBufs p, uint64_t seed_mix,
+                                                                        const uint64_t *base, uint64_t ord, int per_unit) {
+    policy_kernel_body<EXT, MT, LT>(c, b, p, policy_call_key(seed_mix, base, ord), per_unit);
+}
+// aie_rollout_replay_begin: the handle's policy-sampler call count into its device counter, on the replay's stream
+__global__ void __launch_bounds__(32) aie_set_counter_kernel(uint64_t *dst, uint64_t v) {
+    if (threadIdx.x == 0) *dst = v;
+}
 
 // Evaluation of stored actions (aie_evaluate_policy, aie_evaluate_policy_backward): per_unit 0: one warp per row,
 // 1: one warp per (row, unit), units = A + n_act_p; MT: the masks' element type, LT: the logits' and gradients'.
@@ -1022,6 +1049,44 @@ int launch_policy(aie_env *env, const PolicyBufs &p, int lt_bf16, uint64_t sd, v
     env->launches++;
     return AIE_OK;
 }
+// launch_policy's shape with the key read on the device (aie_sample_policy_counter_kernel)
+int launch_policy_counter(aie_env *env, const PolicyBufs &p, int lt_bf16, uint64_t seed_mix, const uint64_t *base,
+                          uint64_t ord, void *stream) {
+    const DevCfg &c = env->cfg;
+    const int units = c.A + (c.planner_acts ? c.B : 0);
+    int per_unit = (c.A * (c.multi_action ? c.n_sub : 1) >= POLICY_PER_UNIT_MIN) ? 1 : 0;
+    if (const char *v = getenv("AIE_POLICY_PER_UNIT")) per_unit = atoi(v) ? 1 : 0;
+    const long long warps = (long long)env->n_envs * (per_unit ? units : 1);
+    const unsigned grid = (unsigned)((warps + 7) / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+#define AIE_POLICY_LAUNCH(MT, LT)                                                                                            \
+    (c.ext ? aie_sample_policy_counter_kernel<true, MT, LT><<<grid, 256, 0, st>>>(c, env->bufs, p, seed_mix, base, ord, per_unit) \
+           : aie_sample_policy_counter_kernel<false, MT, LT><<<grid, 256, 0, st>>>(c, env->bufs, p, seed_mix, base, ord, per_unit))
+    if (c.obs_bf16) {
+        if (lt_bf16) AIE_POLICY_LAUNCH(bf16_t, bf16_t);
+        else AIE_POLICY_LAUNCH(bf16_t, float);
+    } else if (lt_bf16) AIE_POLICY_LAUNCH(float, bf16_t);
+    else AIE_POLICY_LAUNCH(float, float);
+#undef AIE_POLICY_LAUNCH
+    AIE_CUDA(cudaGetLastError(), "aie_sample_policy_counter_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+int launch_set_counter(uint64_t *dst, uint64_t v, void *stream) {
+    aie_set_counter_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(dst, v);
+    AIE_CUDA(cudaGetLastError(), "aie_set_counter_kernel launch");
+    return AIE_OK;
+}
+// A stream that is being captured into a CUDA graph (an error of the query, e.g. the legacy stream while another stream
+// captures, counts as captured: the call is refused rather than recorded)
+bool stream_capturing(void *stream) {
+    cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing((cudaStream_t)stream, &s) != cudaSuccess) {
+        cudaGetLastError();
+        return true;
+    }
+    return s != cudaStreamCaptureStatusNone;
+}
 
 // Row count times units over eight warps per CTA must fit the grid's x dimension.
 static int eval_grid(long long n_rows, int units, unsigned &grid) {
@@ -1141,6 +1206,24 @@ __global__ void __launch_bounds__(256) aie_covid_sample_policy_kernel(const __gr
                                                                       const PolicyBufs p, uint64_t sd) {
     covid_sample_policy_body<LT, MT>(c, b, p, sd);
 }
+// The policy sampler of a captured rollout (aie_rollout_capture_begin): the key read on the device (policy_call_key).
+template <typename LT, typename MT>
+__global__ void __launch_bounds__(256) aie_covid_sample_policy_counter_kernel(const __grid_constant__ CovidCfg c,
+                                                                              const CovidBufs b, const PolicyBufs p,
+                                                                              uint64_t seed_mix, const uint64_t *base,
+                                                                              uint64_t ord) {
+    covid_sample_policy_body<LT, MT>(c, b, p, policy_call_key(seed_mix, base, ord));
+}
+// The step of a captured rollout with final slots bound (aie_rollout_capture_begin): covid_step_env's SLOT variant,
+// launched on every step of the capture; the step that ends an episode finds its final row on the device.
+template <typename OT, bool STATS>
+__global__ void __launch_bounds__(64) aie_covid_step_slot_kernel(const __grid_constant__ CovidCfg c, const CovidBufs b,
+                                                                 const CovidBufs fin, const int32_t *done0, int s, int nk,
+                                                                 const __grid_constant__ CovidStats m) {
+    __shared__ float red[3 * 64];
+    __shared__ uint32_t chg[64 * CV_CHG_CAP];
+    covid_step_env<true, OT, STATS, true>(c, blockIdx.x, b, fin, red, chg, threadIdx.x, blockDim.x, &m, done0, s, nk);
+}
 
 // Evaluation of stored actions (aie_covid_evaluate_policy, *_backward): one warp per (row, unit), units = S + 1.
 template <bool BWD, typename MT, typename LT>
@@ -1203,6 +1286,33 @@ int covid_launch_policy(aie_covid_env *env, const PolicyBufs &p, int lt_bf16, ui
     } else if (lt_bf16) aie_covid_sample_policy_kernel<bf16_t><<<grid, 256, 0, st>>>(env->cfg, env->bufs, p, sd);
     else aie_covid_sample_policy_kernel<float><<<grid, 256, 0, st>>>(env->cfg, env->bufs, p, sd);
     AIE_CUDA(cudaGetLastError(), "aie_covid_sample_policy_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+int covid_launch_policy_counter(aie_covid_env *env, const PolicyBufs &p, int lt_bf16, uint64_t seed_mix, const uint64_t *base,
+                                uint64_t ord, void *stream) {
+    const unsigned grid = (unsigned)(((long long)env->n_envs * (env->cfg.S + 1) + 7) / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+#define AIE_COVID_POLICY(LT, MT) aie_covid_sample_policy_counter_kernel<LT, MT><<<grid, 256, 0, st>>>(env->cfg, env->bufs, p, seed_mix, base, ord)
+    if (env->obs_bf16) {
+        if (lt_bf16) AIE_COVID_POLICY(bf16_t, bf16_t);
+        else AIE_COVID_POLICY(float, bf16_t);
+    } else if (lt_bf16) AIE_COVID_POLICY(bf16_t, float);
+    else AIE_COVID_POLICY(float, float);
+#undef AIE_COVID_POLICY
+    AIE_CUDA(cudaGetLastError(), "aie_covid_sample_policy_counter_kernel launch");
+    env->launches++;
+    return AIE_OK;
+}
+int covid_launch_step_slot(aie_covid_env *env, const CovidBufs &fin, const int32_t *done0, int s, int K, void *stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    const int n = env->n_envs;
+    if (env->obs_bf16) {
+        if (env->metrics_on) aie_covid_step_slot_kernel<bf16_t, true><<<n, 64, 0, st>>>(env->cfg, env->bufs, fin, done0, s, K, env->stats);
+        else aie_covid_step_slot_kernel<bf16_t, false><<<n, 64, 0, st>>>(env->cfg, env->bufs, fin, done0, s, K, env->stats);
+    } else if (env->metrics_on) aie_covid_step_slot_kernel<float, true><<<n, 64, 0, st>>>(env->cfg, env->bufs, fin, done0, s, K, env->stats);
+    else aie_covid_step_slot_kernel<float, false><<<n, 64, 0, st>>>(env->cfg, env->bufs, fin, done0, s, K, env->stats);
+    AIE_CUDA(cudaGetLastError(), "aie_covid_step_slot_kernel launch");
     env->launches++;
     return AIE_OK;
 }

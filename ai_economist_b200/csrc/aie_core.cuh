@@ -1527,6 +1527,13 @@ AIE_DEV uint64_t mix64(uint64_t x) {  // splitmix64 finaliser
     x = (x ^ (x >> 27)) * 0x94d049bb133111ebull;
     return x ^ (x >> 31);
 }
+// The policy sampler's stream key of a call inside a captured rollout (aie_rollout_capture_begin): seed_mix =
+// host_mix64(seed), *base = the handle's policy_calls when the replay began (written on the stream by
+// aie_rollout_replay_begin), ord = the call's ordinal since the capture began.  Call n of an eager loop has the key
+// host_mix64(seed) ^ host_mix64(n), so a replay draws what the same calls made eagerly would.
+AIE_DEV uint64_t policy_call_key(uint64_t seed_mix, const uint64_t *base, uint64_t ord) {
+    return seed_mix ^ mix64(*base + ord + 1);
+}
 // Uniform choice among the set entries of mask[0..n) by one warp: ballots count the open entries, a hashed
 // rank picks one, and the lane holding it is found with popcounts.  Returns the same value on every lane.
 // (masks are 0 / 1: any non-zero element is open; MT: float or bf16_t)

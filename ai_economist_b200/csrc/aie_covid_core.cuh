@@ -239,9 +239,14 @@ constexpr int CV_CHG_CAP = 32;
 // auto-reset, write the sums with this step's values to the previous block, with the end state, and zero the current
 // one.  Each state's thread owns its columns and thread 0 the planner's, so no reduction across states.  ms is unused
 // without STATS.
-template <bool FINAL, typename OT = float, bool STATS = false>
+// SLOT (a step of a captured rollout, aie_rollout_capture_begin): fin's pointers are at row 0 of a bound rollout's final
+// slots and done0 at slot 0 of its done flags; the step that ends an episode (known from the record's own t) writes its
+// final observations into row (k, e), k = the replica's done flags in slots 0 .. s - 1, when k < nk.  Nothing here
+// depends on a host-side timestep or episode count, so a replay at any point of the episode writes the right row.
+template <bool FINAL, typename OT = float, bool STATS = false, bool SLOT = false>
 CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const CovidBufs &fin, float *red, uint32_t *chg,
-                           int tid, int nthr, const CovidStats *ms = nullptr) {
+                           int tid, int nthr, const CovidStats *ms = nullptr, const int32_t *done0 = nullptr, int s = 0,
+                           int nk = 0) {
     const int S = c.S, L = c.L, L1 = c.L + 1, F = c.F;
     float *st = b.state + (size_t)e * CVS_FIELDS * S;
     int32_t *ints = b.ints + (size_t)e * 2 * S;
@@ -453,7 +458,26 @@ CV_DEV void covid_step_env(const CovidCfg &c, int e, const CovidBufs &b, const C
         hdr[CVH_T] = t; hdr[CVH_SUBSIDY_LEVEL] = level; hdr[CVH_RING_HEAD] = new_head;
     }
     cv_bsync();
-    if (FINAL) {
+    if (SLOT) {
+        const bool end = c.auto_reset && t >= c.T;   // uniform across the CTA: t is the replica's
+        int k = 0;
+        if (end) {
+#if CV_ON_DEVICE
+            for (int t0 = 0; t0 < s; t0 += nthr) {
+                const int u = t0 + tid;
+                k += __syncthreads_count(u < s && done0[(size_t)u * c.n_envs + e] != 0);
+            }
+#else
+            for (int u = 0; u < s; u++) k += done0[(size_t)u * c.n_envs + e] != 0;
+#endif
+        }
+        if (end && k < nk) {
+            covid_observe<OT>(c, st, ints, hdr, ring, new_head, k * c.n_envs + e, fin, tid, nthr);
+            cv_bsync();   // the reset below overwrites what the final pass reads
+        }
+        if (end) covid_reset_env<OT>(c, e, b, tid, nthr, true);
+        else covid_observe<OT>(c, st, ints, hdr, ring, new_head, e, b, tid, nthr);
+    } else if (FINAL) {
         // One observation pass whose destination is chosen per step: a second inlined pass for the ending step made
         // the ordinary steps of this kernel 7.7 % slower on an H100 (the code ptxas makes of the whole body); this form
         // leaves them unchanged (DESIGN §6).

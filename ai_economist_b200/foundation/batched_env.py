@@ -15,6 +15,7 @@ import ctypes as C
 import numpy as np
 
 from .agents import agent_registry
+from . import rollout_graph as _rg
 from .components import component_registry
 from .entities import endogenous_registry, landmark_registry, resource_registry
 
@@ -376,6 +377,9 @@ class BatchedFoundationEnv:
     def reset(self, seed_state=None, force_dense_logging=False):
         """seed_state: optional numpy stream state(s) to start the reset from (base_env.py:873-884) - one 5-tuple (every
         replica when n_envs == 1, else replica 0) or a list with one 5-tuple per replica."""
+        _rg.refuse_in_act(self, "reset")
+        if self._rollout is not None and self._stepper.rollout_slot != 0:
+            _rg.invalidate(self)   # refused below: the graph's rollout was left mid-way
         if self._loaded and "episode_final" not in self._stepper.buf and self._episode_finished(0):
             # base_env.py:763-765, 1022-1025: _finalize_logs stores the metrics only on the step that ENDS an episode, so
             # resetting an unfinished episode (or resetting twice) leaves previous_episode_metrics untouched
@@ -538,6 +542,7 @@ class BatchedFoundationEnv:
         """actions: None (all NO-OP) | reference-style dict {agent_idx: action(s)} with a leading env axis |
         tensor [E, A, n_act] | (agent_actions, planner_actions).  Writing straight into
         `env.action_buffers` and calling step(env.action_buffers) avoids any copy."""
+        _rg.refuse_in_act(self, "step")
         assert self._loaded, "call reset() first"
         self._write_actions(actions)
         lg = self._dense_logger
@@ -588,6 +593,8 @@ class BatchedFoundationEnv:
         unbind_rollout() returns to the env's own buffers.  Dense logging (it reads replica 0's bound action, reward
         and done buffers) is refused with a ValueError, a stepper_factory whose stepper cannot bind rollouts with
         NotImplementedError."""
+        _rg.refuse_in_act(self, "bind_rollout")
+        _rg.invalidate(self)
         st = self._stepper
         if not hasattr(st, "bind_rollout"):
             raise NotImplementedError("this env's stepper cannot bind rollouts")
@@ -617,13 +624,39 @@ class BatchedFoundationEnv:
 
     def restart_rollout(self):
         """Start the next rollout in the bound tensors (after its T steps): slot T's observations move to slot 0."""
+        _rg.refuse_in_act(self, "restart_rollout")
         if self._rollout is None:
             raise ValueError("no rollout bound")
         self._stepper.restart_rollout()
         self._aim_rollout()
 
+    def capture_rollout(self, act):
+        """Record the bound rollout's T steps once as a CUDA graph and return a RolloutGraph whose replay() runs them
+        again: for t in range(T), act(t, rollout.obs_slots[t]) then step(env.action_buffers).
+
+        act: the policy's part of a step, torch ops on the env's device plus at most sample_actions (any other env call
+        inside it is a ValueError).  It must not synchronise with the host or branch on device values, and its outputs
+        should go to tensors that outlive the capture (e.g. per-slot rows of the trainer's buffers).  Needs a bound
+        rollout at slot 0 after reset(), and the CUDA stepper (NotImplementedError otherwise).  Before recording, act
+        runs once at slot 0 as torch's warm-up; the sampler's draws and the slot's actions it wrote are given back.
+        Recording executes nothing: the env's counters, cursor and buffers are as they were before the call.
+
+        replay() needs cursor 0 (after reset() or restart_rollout()) and leaves it at T, with every output what the
+        eager loop leaves from the same state, byte for byte, when act is bit-reproducible under capture: the policy
+        sampler reads its call count on the device, so draws differ from replay to replay as they do eagerly; the seed
+        passed to sample_actions is fixed at capture.  Tensors are read by address, so in-place updates of the policy's
+        weights are seen.  Eager rollouts may run between replays.  Unbinding or re-binding the rollout,
+        load_state_dict() and reset() attempted mid-rollout invalidate the graph (replay() raises ValueError), as does
+        capturing again.  Refused with ValueError under the Saez tax model, whose host-side estimator runs after every
+        step.  The launch count includes the warm-up's launches."""
+        if self._saez is not None:
+            raise ValueError("capture_rollout: the Saez tax model runs its estimator on the host after every step")
+        return _rg.capture_rollout(self, act)
+
     def unbind_rollout(self):
         """Back to the env's own buffers (env.obs, env.rew, ... as before bind_rollout)."""
+        _rg.refuse_in_act(self, "unbind_rollout")
+        _rg.invalidate(self)
         if self._rollout is None:
             return
         self._stepper.unbind_rollout()
@@ -668,6 +701,7 @@ class BatchedFoundationEnv:
         respect to both logits tensors: the backward is one device launch that recomputes the softmax.  A segment
         with nothing open gives 0 and 0 (gradient 0); a NaN or +inf open logit, no finite open logit, or a stored
         action that is closed gives NaN (see include/aie_b200.h).  Asynchronous; the env's state is not touched."""
+        _rg.refuse_in_act(self, "evaluate_actions")
         return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
 
     def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0,
@@ -690,6 +724,7 @@ class BatchedFoundationEnv:
         A bound rollout's storage is taken as it is: rewards = rollout.buf["reward"] [T, E, A + 1] (split here with one
         copy per group), dones = rollout.buf["done"], and with per_episode_end=True final_values [K, E, A] / [K, E], the
         values of the final slots: a done step reads the row of its episode-end ordinal in its replica (0 for the first)."""
+        _rg.refuse_in_act(self, "compute_advantages")
         return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam,
                                                 per_episode_end=per_episode_end)
 
@@ -726,6 +761,7 @@ class BatchedFoundationEnv:
         recorded and the host-side tables drawn at construction.  Observations are not stored (except under the Saez
         tax model): load_state_dict() re-derives them from the records.  Allowed after the first reset(); with a rollout
         bound only at slot 0 (ValueError otherwise)."""
+        _rg.refuse_in_act(self, "state_dict")
         from . import checkpoint as ck
         if not self._loaded:
             raise ValueError("state_dict: nothing to save before the first reset()")
@@ -759,6 +795,8 @@ class BatchedFoundationEnv:
         From here on every call returns what
         it would have returned in the env the dict was taken from.  Allowed on a new env before any reset(), and between
         steps; with a rollout bound only at slot 0 (the observations go into slot 0)."""
+        _rg.refuse_in_act(self, "load_state_dict")
+        _rg.invalidate(self)
         from . import checkpoint as ck
         ck.check_config(sd, self._checkpoint_config())
         ck.refuse_mid_rollout(self, "load_state_dict")
@@ -928,11 +966,13 @@ class BatchedFoundationEnv:
     @property
     def metrics(self):
         """The combined scenario + component metrics of env 0 (BaseEnvironment.metrics, base_env.py:421-432)."""
+        _rg.refuse_in_act(self, "metrics")
         return self.metrics_of(0)
 
     def metrics_of(self, e, _count_finished=True):
         """`env.metrics` of replica e: layout_from_file.py:595-650 + every component's get_metrics(), computed from the
         replica's state record (the event logs are device-side running sums, see foundation/metrics.py)."""
+        _rg.refuse_in_act(self, "metrics_of")
         from .metrics import metrics_from_state
         st = self._stepper.read_state(e)
         if _count_finished and int(np.asarray(st["t"]).reshape(-1)[0]) >= self._episode_length:
@@ -946,9 +986,11 @@ class BatchedFoundationEnv:
     @property
     def previous_episode_metrics(self):
         """Metrics of the episode env 0 finished last (base_env.py:414-418); None before the first auto-reset."""
+        _rg.refuse_in_act(self, "previous_episode_metrics")
         return self.previous_episode_metrics_of(0)
 
     def previous_episode_metrics_of(self, e):
+        _rg.refuse_in_act(self, "previous_episode_metrics_of")
         from .metrics import metrics_from_state
         st = self._stepper
         if "episode_final" not in st.buf:   # no auto-reset: what the last explicit reset() stored (replica 0 only)
@@ -971,6 +1013,7 @@ class BatchedFoundationEnv:
         the curves it logs (productivity, equality, trades, tax rates) without stalling the stream, e.g.
         `env.metrics_tensor()[:, env.metric_keys.index("social/productivity")].mean()`.  out: an optional preallocated
         contiguous float64 [n_envs, K] tensor."""
+        _rg.refuse_in_act(self, "metrics_tensor")
         m = self._stepper.episode_metrics(final=False, out=out)
         if self._saez is not None:
             self._fill_saez_elasticity(m, np.asarray(self._saez.batch.elas_tm1, np.float64))
@@ -982,6 +1025,7 @@ class BatchedFoundationEnv:
         Needs auto_reset (the end-of-episode records); without it the library's AieError is raised.  Training-loop idiom,
         the metrics of the episodes that ended in this step with no synchronisation until the caller reduces them:
             m = env.previous_episode_metrics_tensor(); logged = m[env.done["__all__"].bool()]"""
+        _rg.refuse_in_act(self, "previous_episode_metrics_tensor")
         m = self._stepper.episode_metrics(final=True, out=out)
         if self._saez is not None:
             ends = self._saez.elas_at_episode_end

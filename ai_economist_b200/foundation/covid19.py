@@ -16,6 +16,7 @@ from datetime import datetime
 import numpy as np
 
 from .._abi import COVID_OBS_NAMES
+from . import rollout_graph as _rg
 
 DATA_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "covid19_data")
 F32, I32 = np.float32, np.int32
@@ -333,6 +334,8 @@ class CovidBatchedEnv:
         step's slot, step() advances s and reset() is allowed only at s == 0; env.final_obs is not written.  After T
         steps, restart_rollout() carries slot T into slot 0.  A stepper_factory whose stepper cannot bind rollouts is
         refused with NotImplementedError."""
+        _rg.refuse_in_act(self, "bind_rollout")
+        _rg.invalidate(self)
         st = self._stepper
         if not hasattr(st, "bind_rollout"):
             raise NotImplementedError("this env's stepper cannot bind rollouts")
@@ -370,6 +373,7 @@ class CovidBatchedEnv:
 
     def restart_rollout(self):
         """Start the next rollout in the bound tensors (after its T steps): slot T moves to slot 0."""
+        _rg.refuse_in_act(self, "restart_rollout")
         if self._rollout is None:
             raise ValueError("no rollout bound")
         self._stepper.restart_rollout()
@@ -379,7 +383,16 @@ class CovidBatchedEnv:
             r.buf["rate_planner"][0][...] = r.buf["rate_planner"][r.T]
         self._aim_rollout()
 
+    def capture_rollout(self, act):
+        """Record the bound rollout's T steps once as a CUDA graph (the contract of
+        BatchedFoundationEnv.capture_rollout).  The step finds the final-slot row of an episode end on the device, and
+        under VaccinationCampaign(observe_rate=True) the rate lookups are device-side torch ops of each slot, recorded
+        with the step."""
+        return _rg.capture_rollout(self, act)
+
     def unbind_rollout(self):
+        _rg.refuse_in_act(self, "unbind_rollout")
+        _rg.invalidate(self)
         if self._rollout is None:
             return
         self._stepper.unbind_rollout()
@@ -419,6 +432,7 @@ class CovidBatchedEnv:
         [*B, 1 + levels, 51] as obs["a"]["action_mask"], mask_planner [*B, 1 + subsidy levels]); actions =
         (actions_agent [*B, 51], actions_planner [*B]), int32.  Returns (log_prob_agent [*B, 51], log_prob_planner
         [*B], entropy_agent [*B, 51], entropy_planner [*B]), differentiable with respect to both logits tensors."""
+        _rg.refuse_in_act(self, "evaluate_actions")
         return self._stepper.evaluate_actions(logits_agent, logits_planner, actions, masks)
 
     def compute_advantages(self, rewards, values, dones, last_values, final_values=None, *, gamma, lam=1.0,
@@ -430,6 +444,7 @@ class CovidBatchedEnv:
         (env created with final_obs=True) bootstraps it; final_values=None treats an episode end as terminal.  A bound
         rollout: (rollout.buf["reward_agent"], rollout.buf["reward_planner"]), rollout.buf["done"] and, with
         per_episode_end=True, the values of its [K, ...] final slots."""
+        _rg.refuse_in_act(self, "compute_advantages")
         return self._stepper.compute_advantages(rewards, values, dones, last_values, final_values, gamma=gamma, lam=lam,
                                                 per_episode_end=per_episode_end)
 
@@ -455,12 +470,14 @@ class CovidBatchedEnv:
         """scenario_metrics() of every replica's running episode as one float64 tensor [n_envs, K] on the device (columns:
         metric_keys), one kernel launch, no synchronisation.  Mid-episode the time means divide by episode_length, as the
         reference's zero-padded global_state does.  out: an optional contiguous float64 [n_envs, K] tensor."""
+        _rg.refuse_in_act(self, "metrics_tensor")
         self._need_metrics()
         return self._stepper.episode_metrics(final=False, out=out)
 
     def previous_episode_metrics_tensor(self, out=None):
         """scenario_metrics() of the episode every replica finished last, float64 [n_envs, K] on the device, one launch.
         Before any episode has ended the library's AieError is raised (previous_episode_metrics is None then)."""
+        _rg.refuse_in_act(self, "previous_episode_metrics_tensor")
         self._need_metrics()
         return self._stepper.episode_metrics(final=True, out=out)
 
@@ -476,17 +493,21 @@ class CovidBatchedEnv:
     @property
     def metrics(self):
         """scenario_metrics() of replica 0's running episode (BaseEnvironment.metrics)."""
+        _rg.refuse_in_act(self, "metrics")
         return self.metrics_of(0)
 
     def metrics_of(self, e):
+        _rg.refuse_in_act(self, "metrics_of")
         return self.metrics_rows_as_dicts(self.metrics_tensor(), envs=[e])[0]
 
     @property
     def previous_episode_metrics(self):
         """scenario_metrics() of the episode replica 0 finished last; None before any has ended."""
+        _rg.refuse_in_act(self, "previous_episode_metrics")
         return self.previous_episode_metrics_of(0)
 
     def previous_episode_metrics_of(self, e):
+        _rg.refuse_in_act(self, "previous_episode_metrics_of")
         self._need_metrics()
         if not self._stepper.has_previous_episode():
             return None
@@ -641,6 +662,7 @@ class CovidBatchedEnv:
         simulation buffers, observations, rewards, actions, final observations and metric accumulators (copies on the
         env's device), the library's sampler counters and the lock-step timestep.  Allowed after the first reset();
         with a rollout bound only at slot 0 (ValueError otherwise)."""
+        _rg.refuse_in_act(self, "state_dict")
         from . import checkpoint as ck
         if not self._loaded:
             raise ValueError("state_dict: nothing to save before the first reset()")
@@ -655,6 +677,8 @@ class CovidBatchedEnv:
         """Load a state_dict() taken from an env of the same configuration (ValueError naming the field that differs)
         into this env's own buffers; with a rollout bound only at slot 0, whose observations it writes.  Allowed on a
         new env before any reset()."""
+        _rg.refuse_in_act(self, "load_state_dict")
+        _rg.invalidate(self)
         from . import checkpoint as ck
         ck.check_config(sd, self._checkpoint_config())
         ck.refuse_mid_rollout(self, "load_state_dict")
@@ -669,6 +693,9 @@ class CovidBatchedEnv:
         return self.obs
 
     def reset(self):
+        _rg.refuse_in_act(self, "reset")
+        if self._rollout is not None and self._stepper.rollout_slot != 0:
+            _rg.invalidate(self)   # refused below: the graph's rollout was left mid-way
         self._stepper.reset()
         self._loaded = True
         if self._rollout is not None:
@@ -678,6 +705,7 @@ class CovidBatchedEnv:
 
     def step(self, actions=None):
         """actions: None | {"a": int tensor [E, 51], "p": int tensor [E]} | (agent_actions, planner_actions)."""
+        _rg.refuse_in_act(self, "step")
         assert self._loaded, "call reset() first"
         ba, bp = self.action_buffers
         if actions is None:

@@ -136,6 +136,40 @@ class PolicySampler:
         self._check(self._policy_fn(self._h, C.byref(p), C.c_uint64(int(seed)), self._stream()))
         return lp_a, lp_p
 
+    # -- captured rollouts (aie_rollout_capture_begin ... / aie_covid_rollout_capture_begin ...) ----------------------
+    # The stepper provides _capture_prefix ("aie" | "aie_covid"); the four calls keep rollout_slot in step with the
+    # library's cursor.  A stepper that can record CUDA graphs sets supports_rollout_capture.
+    supports_rollout_capture = False
+
+    def _capture_fn(self, name):
+        return getattr(self.lib, "%s_rollout_%s" % (self._capture_prefix, name))
+
+    def rollout_capture_begin(self):
+        """Start recording the bound rollout (slot 0): until rollout_capture_end() only step() and sample_policy() run."""
+        self._check(self._capture_fn("capture_begin")(self._h, self._stream()))
+        self._capturing = True
+
+    def rollout_capture_end(self):
+        """Stop recording: the library's host state and the cursor are as they were at rollout_capture_begin()."""
+        self._capturing = False
+        self._check(self._capture_fn("capture_end")(self._h))
+        self.rollout_slot = 0
+
+    def rollout_replay_begin(self):
+        """Before a replay (cursor 0): the current call counter into the device counter, on the stream."""
+        self._check(self._capture_fn("replay_begin")(self._h, self._stream()))
+
+    def rollout_replay_end(self):
+        """After a replay: the library's host state advanced by what the captured calls did; the cursor at T."""
+        self._check(self._capture_fn("replay_end")(self._h))
+        self.rollout_slot = self.rollout.T
+
+    def _refused_in_capture(self, rc):
+        """A call the library refused because a rollout is being recorded (only the step and the policy sampler run)."""
+        if rc == _abi.AIE_ESTATE and getattr(self, "_capturing", False):
+            raise ValueError("not available while a rollout is being captured (capture_rollout's act may call "
+                             "sample_actions only): %s" % self.lib.aie_last_error().decode())
+
     # -- evaluation of stored actions (aie_evaluate_policy / aie_covid_evaluate_policy and their backward) -----------
     def _eval_args(self, logits_agent, logits_planner, actions, masks, grads=()):
         """Validate the inputs of an evaluation; returns (aie_policy_eval with the inputs set, leading shape, row
@@ -478,7 +512,10 @@ class BatchStepper(PolicySampler):
     # --------------------------------------------------------------------------------------------------
     def _check(self, rc):
         if rc != _abi.AIE_OK:
+            self._refused_in_capture(rc)
             raise _abi.AieError("aie error %d: %s" % (rc, self.lib.aie_last_error().decode()))
+
+    _capture_prefix = "aie"
 
     def close(self):
         if getattr(self, "_h", None):
@@ -807,6 +844,7 @@ class CudaStepper(BatchStepper):
     """The product path: torch-owned CUDA tensors, kernels launched on torch's current stream."""
 
     _TORCH = None
+    supports_rollout_capture = True
 
     def __init__(self, spec, n_envs, device="cuda:0", auto_reset=True, lib_path=None, event_envs=0):
         import torch

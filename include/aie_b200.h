@@ -627,6 +627,37 @@ typedef struct aie_counters {
 int aie_get_counters(aie_env *env, aie_counters *out);
 int aie_set_counters(aie_env *env, const aie_counters *in);
 
+/* ABI 6 (additive).  A bound rollout recorded once as a CUDA graph and replayed (torch.cuda.graph, cudaStreamBeginCapture).
+ * A replay repeats the launches' arguments as they were at capture, so nothing a launch takes from the host may change
+ * between replays.  The gather-trade-build step takes only the slot's pointers (fixed per slot) and the final pass
+ * finds its row from the stored done flags on the device; what remains is the policy sampler's key, which counts calls
+ * on the host.  Between aie_rollout_capture_begin and aie_rollout_capture_end, aie_sample_policy launches
+ * aie_sample_policy_counter_kernel, whose key is host_mix64(seed) ^ host_mix64(base + i + 1): base is read on the device
+ * from the handle's call counter, i is the call's ordinal since capture_begin, baked into the launch.  That is the key
+ * of call base + i + 1 of an eager loop, so a replay draws what the same calls made eagerly from the same state would.
+ *
+ * aie_rollout_capture_begin: needs a bound rollout at slot 0.  Allocates the handle's device counter (16 bytes, once,
+ * before any capture is opened: nothing may allocate inside one), writes policy_calls into it on `stream`, saves the
+ * host state (slot cursor, policy_calls, launch count) and switches aie_sample_policy to the variant above.  Between it
+ * and aie_rollout_capture_end only aie_step and aie_sample_policy are allowed (every other entry point of the handle is
+ * AIE_ESTATE); the caller opens and closes the stream capture inside the pair.  aie_rollout_capture_end records what the
+ * captured calls did (steps, sampler calls, launches) and puts the saved host state back: nothing was executed.
+ * aie_rollout_replay_begin: needs slot 0 and a capture in the bound rollout (aie_bind_rollout, bind or unbind, drops
+ * it); writes the current policy_calls into the device counter with one launch on `stream`, which the caller then
+ * replays the graph on.  aie_rollout_replay_end applies the recorded deltas: s = the captured steps (T), policy_calls
+ * += the captured sampler calls, the launch count += the captured launches.  Eager rollouts may run between replays.
+ *
+ * A capture opened without the pair is refused rather than recorded wrong: aie_step, aie_sample_policy,
+ * aie_sample_random_actions, aie_set_fused_policy, aie_reset_envs, aie_load_state, aie_rollout_restart and the pair's
+ * own calls return AIE_ESTATE when their stream is being captured outside capture_begin / capture_end (the check is one
+ * cudaStreamIsCapturing query; uncaptured calls are unchanged).
+ * AIE_EINVAL for a NULL env; AIE_ESTATE as above, for a second capture_begin before capture_end, capture_end without
+ * capture_begin, and replay_end without replay_begin; AIE_ENOMEM if the counter cannot be allocated. */
+int aie_rollout_capture_begin(aie_env *env, void *stream);
+int aie_rollout_capture_end(aie_env *env);
+int aie_rollout_replay_begin(aie_env *env, void *stream);
+int aie_rollout_replay_end(aie_env *env);
+
 /* ================================================================================================
  * COVID-19 + economy scenario (BASELINE config 4)
  *
@@ -823,6 +854,21 @@ typedef struct aie_covid_counters {
 } aie_covid_counters;
 int aie_covid_get_counters(aie_covid_env *env, aie_covid_counters *out);
 int aie_covid_set_counters(aie_covid_env *env, const aie_covid_counters *in);
+
+/* ABI 6 (additive).  A captured rollout of the COVID-19 scenario: the contract of aie_rollout_capture_begin and its three
+ * companions, with aie_covid_step and aie_covid_sample_policy the calls allowed inside the pair (aie_covid_sample_policy
+ * launches aie_covid_sample_policy_counter_kernel, keyed as the gather-trade-build one).  The eager step picks the final
+ * row k and the kernel from the host's lock-step timestep; inside the pair, with final slots bound, every step launches
+ * aie_covid_step_slot_kernel instead, which finds the step that ends an episode from the record's own t and the row k
+ * from the replica's done flags in slots 0 .. s - 1 of the rollout (the ordinal the gather-trade-build final pass uses).
+ * capture_begin also saves the timestep, the episode-end count of the rollout and the previous-episode flag, and
+ * capture_end puts them back; aie_covid_rollout_replay_end advances them as T eager steps would (every replica ends an
+ * episode on the same step).  Refused on a capture opened without the pair: aie_covid_step, aie_covid_step_final,
+ * aie_covid_sample_policy, aie_covid_sample_random_actions, aie_covid_reset, aie_covid_rollout_restart. */
+int aie_covid_rollout_capture_begin(aie_covid_env *env, void *stream);
+int aie_covid_rollout_capture_end(aie_covid_env *env);
+int aie_covid_rollout_replay_begin(aie_covid_env *env, void *stream);
+int aie_covid_rollout_replay_end(aie_covid_env *env);
 
 const char *aie_last_error(void);
 int aie_abi_version(void);
